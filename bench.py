@@ -17,7 +17,7 @@ content, files warm in tmpfs/page cache.  A "step" = one pass of the hot path ov
 * `roofline`: dominant kernel kk_convert_kernel.  N = 1: bound "hbm", algorithmic bytes = 2 x shard bytes (2 B read + 2 B written
   per bf16 element) / its CUDA-event duration, against MEASURED_PEAKS.json's hbm_gbs.  N > 1 broadcast: bound "nvlink", the
   bytes every GPU has to receive ((N-1)/N of the pool) / the fan-out stage's CUDA-event time, against a peer-copy rate measured
-  in the same run (every rank reading from its ring neighbour at once, kk_probe_peer) and against 900 GB/s nominal.
+  in the same run (every rank reading from its ring neighbour at once, kk_probe_peer) and against H100 NVLink 4's 450 GB/s per direction.
 * `cpu_baseline`: the oracle's C port (oracle/kk_oracle.c, OpenMP, all host threads) over the WHOLE checkpoint.
 * `secondary` (N = 1, default workload): the same kernel stage on a 4-layer Mixtral q4_K GGUF — the expanding conversion for which
   the north_star's HBM-write fraction is meaningful (a bf16 copy has to read what it writes and tops out near 0.5 of it).
@@ -46,6 +46,10 @@ import numpy as np  # noqa: E402
 
 METRIC = "model_load_GBps"
 UNIT = "GB/s"
+MIXTRAL_STAGE_LAYERS = 16
+H100_HBM_GBPS = 3350.0  # H100 SXM data sheet, HBM3
+H100_NVLINK_GBPS = 450.0  # H100 SXM NVLink 4, per direction (900 GB/s both directions together)
+DUMP_MAX_BYTES = 64 << 20
 
 
 def parse():
@@ -62,6 +66,8 @@ def parse():
     ap.add_argument("--gen-only", action="store_true", help="internal: write the synthetic checkpoint into --data-dir and exit (run as a child process by make_files)")
     ap.add_argument("--no-interleave", action="store_true", help="do not spread the synthetic files' page-cache pages over the NUMA nodes")
     ap.add_argument("--keep-data", action="store_true")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR", help="after the timed steps, write what the last timed step left in the pool to "
+                    "DIR/<tensor name>.npy: every tensor, floats as float32, integers as float64, whole or as a fixed seeded sample, at most 64 MiB in all")
     ap.add_argument("--readers", type=int, default=0)
     ap.add_argument("--slots", type=int, default=0)
     ap.add_argument("--slot-mb", type=int, default=0)
@@ -79,12 +85,12 @@ def parse():
     ap.add_argument("--no-secondary", action="store_true", help="N = 1 default workload: skip the short Mixtral q4_K record (`secondary`)")
     ap.add_argument("--fanout", default="auto", choices=["auto", "p2p", "raw", "pull"],
                     help="broadcast order: fused convert+fan-out by P2P stores (p2p), all-gather the file bytes then convert locally (raw), or convert into own "
-                         "pool + slice buffer and pull the peers' slices (pull: peers map 1/N of the bytes).  auto = p2p (measured best on every count at N = 8)")
+                         "pool + slice buffer and pull the peers' slices (pull: peers map 1/N of the bytes).  auto = p2p")
     a = ap.parse_args()
     if a.fanout == "auto":
-        # Measured at N = 8 (profiles/README.md, round 2): with pools in 2 MiB multiples the seven 16 GB pool mappings of the P2P-store order take
-        # 0.05-0.07 s (3.6 s in round 1), so it has the shorter time-to-ready, the faster kernel stage (20.0 vs 25.2 ms) and the faster e2e step
-        # (156 vs 183 ms: its fan-out overlaps the ingest).  PULL stays available for deployments where peers must not map whole pools.
+        # The P2P-store order converts and fans out in one pass and its fan-out overlaps the ingest; with pools in 2 MiB multiples its peer
+        # mappings are cheap.  Not yet re-timed against PULL and RAW on several H100s.  PULL stays available for deployments where peers must
+        # not map whole pools.
         a.fanout = "p2p"
     return a
 
@@ -109,11 +115,14 @@ def workload_spec(args):
         name = "Llama-3-70B bf16 safetensors scatter" + (f" (REDUCED to {args.layers} layers)" if args.layers else "")
         return dict(kind="llama", cfg=cfg, tensors=t, name=name, mode="scatter")
     if args.workload == "mixtral-q4k":
-        kw = dict(layers=args.layers) if args.layers else {}
+        # All 32 layers in bf16 are 93 GB, more than one H100's 80 GB holds: the full-size workload is the first 16 layers (47 GB of bf16 from
+        # 13 GB of blocks), the share of one GPU in a two-stage pipeline split of the model.
+        layers = args.layers or MIXTRAL_STAGE_LAYERS
         if args.qtype not in synth.GGML or synth.GGML[args.qtype][1] == 1:
             raise SystemExit(f"--qtype {args.qtype}: not a block-quantised GGUF type this tool can write")
-        t = synth.mixtral_gguf_tensors(qtype=args.qtype, **kw)
-        name = f"Mixtral-8x7B GGUF {args.qtype.lower()} -> bf16" + (f" (REDUCED to {args.layers} layers)" if args.layers else "")
+        t = synth.mixtral_gguf_tensors(qtype=args.qtype, layers=layers)
+        name = f"Mixtral-8x7B GGUF {args.qtype.lower()} -> bf16" + (f" (REDUCED to {args.layers} layers)" if args.layers else
+                                                                     f" (layers 0-{layers - 1} of 32: one stage of a two-GPU pipeline split)")
         return dict(kind="gguf", tensors=t, name=name, mode="broadcast")
     if args.layers:  # test-sized: the reduced model also gets a 4096-entry vocabulary (wte is 154 of the full model's 498 MB)
         t = synth.gpt2_tensors(n_layer=args.layers, vocab=4096)
@@ -235,8 +244,16 @@ def _write_files(spec, d: str, synth) -> None:
 # ---------------------------------------------------------------------------------------------
 # clocks
 # ---------------------------------------------------------------------------------------------
+def _num(field: str):
+    """A numeric nvidia-smi field, or None where it reports "[N/A]" or similar."""
+    try:
+        return float(field)
+    except ValueError:
+        return None
+
+
 class ClockSampler:
-    Q = "index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
+    Q = "index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,power.limit,name"
 
     def __init__(self, gpu: int):
         self.gpu, self.rows, self.p = gpu, [], None
@@ -265,7 +282,8 @@ class ClockSampler:
         names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
         reasons = sorted({n for r in rows for n, v in zip(names, r[4:8]) if v.lower().startswith("active")})
         return {"sm_mhz": statistics.median(sm), "sm_max_mhz": float(rows[0][2]), "reasons": reasons, "samples": len(rows),
-                "power_w_max": max(float(r[3]) for r in rows)}
+                "power_w_max": max((w for w in (_num(r[3]) for r in rows) if w is not None), default=None), "gpu": rows[0][9] if len(rows[0]) > 9 else None,
+                "power_limit_w": _num(rows[0][8]) if len(rows[0]) > 9 else None}
 
 
 # ---------------------------------------------------------------------------------------------
@@ -274,8 +292,7 @@ class ClockSampler:
 def cpu_port_setup(path: str, sample_bytes: int | None = None):
     """Jobs over the whole checkpoint (sample_bytes None) and an UNTOUCHED output buffer: its pages are first touched by the untimed warm-up
     pass, i.e. by the OpenMP thread that writes them in every later pass (orc_cpu_load schedules jobs statically), so the buffer ends up
-    spread over both sockets.  Round 1 touched it from one thread — everything on one NUMA node — and the same port read 9 GB/s on one box
-    and 50 GB/s on the next."""
+    spread over both sockets.  Touched from one thread, the whole buffer sits on one NUMA node and the rate depends on which one."""
     from oracle import coracle, oracle
     shards, recs = oracle.index_path(path)
     plan, total = oracle.plan_pool(recs)
@@ -406,10 +423,9 @@ def main():
     barrier()
     path = d if spec["kind"] != "gguf" else os.path.join(d, "model.gguf")
     t_gen = time.time() - t_gen
-    # "files warm in the page cache" means they have been READ before, not only written: the first read of freshly written tmpfs pages by 8 x 16
-    # threads is an order of magnitude slower than every later one (measured on a fresh 8-GPU box: 1.33 s of pread per reader thread in the cold
-    # load against 0.11 s when the same files had been loaded once before — profiles/r02/bench_n8_first_vs_second_run.txt; the kernel promotes
-    # pages to the active LRU list on re-reference, under a lock all readers share).  So every rank reads its stripe of the files twice, untimed.
+    # "files warm in the page cache" means they have been READ before, not only written: the first read of freshly written tmpfs pages by many
+    # reader threads is much slower than every later one (the kernel promotes pages to the active LRU list on re-reference, under a lock all
+    # readers share).  So every rank reads its stripe of the files twice, untimed.
     t_warm = time.time()
     warm_page_cache(d, rank, world)
     barrier()
@@ -584,9 +600,8 @@ def main():
     if args.kernel_only:
         e2e_ts = [float("nan")]
     else:
-        # The harness's own garbage collector stays out of the timed steps: a generation-2 pass over a torch-sized heap is 50-150 ms, a third of a
-        # step (it showed as one step in six taking 0.46 s while kk_load_part took its usual 0.30 s, profiles/r02/e2e_read_modes_q.jsonl); a Go or
-        # C++ caller of the C ABI has no such pause.
+        # The harness's own garbage collector stays out of the timed steps: a generation-2 pass over a torch-sized heap takes tens of milliseconds
+        # and lands in whichever step triggers it; a Go or C++ caller of the C ABI has no such pause.
         gc.collect()
         gc.freeze()
         gc.disable()
@@ -612,6 +627,8 @@ def main():
                 "read_mode": os.environ.get("KUKEON_GPULOAD_READ", "auto"), "e2e_ms_each": [t * 1e3 for t in e2e_ts], "steps_detail": step_detail[-args.steps:],
                 "config": {"readers": args.readers, "slots": args.slots, "slot_mb": args.slot_mb, "zerocopy": args.zerocopy, "numa_pin": not args.no_numa_pin,
                            "chunks_per_load": chunks_per_load, "kk_open_s": t_open}}
+        if args.dump_outputs and rank == 0:
+            dump_outputs(m, ref, local, args.dump_outputs)
         m.release()
         pool.close()
         barrier()
@@ -655,6 +672,8 @@ def main():
     wall = time.perf_counter() - wall0
     tc1 = time.time()
     ck = clocks.stop(tc0, tc1)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(m, ref, local, args.dump_outputs)
     dev_ms = allmax(sum(step_ms))
     value = delivered * args.steps / (dev_ms / 1e3) / 1e9
     n_launch = len(launch_ms[0])
@@ -664,7 +683,7 @@ def main():
     pk = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(pk):
         peaks = json.load(open(pk))
-    peak, peak_src = (peaks["hbm_gbs"], "measured (MEASURED_PEAKS.json hbm_gbs, copy read+write)") if "hbm_gbs" in peaks else (6650.0, "fallback (B200_PROFILING.md)")
+    peak, peak_src = (peaks["hbm_gbs"], "measured (MEASURED_PEAKS.json hbm_gbs, copy read+write)") if "hbm_gbs" in peaks else (H100_HBM_GBPS, "H100 SXM data sheet")
     avg_launch_ms = sum(sum(p) for p in launch_ms) / (len(launch_ms) * max(n_launch, 1))
     # algorithmic HBM bytes of this rank per launch: source read once + pool writes landing in THIS GPU's HBM
     alg_per_step = local_src + part["out_bytes"] * (1 if mode == gpupool.MODE_SCATTER else world) if mode != gpupool.MODE_SINGLE else local_src + part["out_bytes"]
@@ -674,19 +693,6 @@ def main():
         alg_per_step = local_src + 2 * part["out_bytes"] + (pool_bytes - part["out_bytes"])
     alg_per_launch = alg_per_step / max(n_launch, 1)
     achieved = alg_per_launch / (avg_launch_ms / 1e3) / 1e9 if avg_launch_ms > 0 else 0.0
-    # DRAM traffic of the dominant kernel from the committed `ncu --set full` capture of THIS kernel build (profiles/traffic.json names the capture and
-    # the build it was taken from): dram__bytes_read.sum + dram__bytes_write.sum of one launch as a ratio to that launch's algorithmic bytes, scaled to
-    # this run's launch.  Never measured inside a timed run (nothing here runs under a profiler).
-    traffic = traffic_src = None
-    tf = os.path.join(ROOT, "profiles", "traffic.json")
-    if os.path.exists(tf) and world == 1:
-        try:
-            key = args.workload if (args.workload != "mixtral-q4k" or args.qtype == "Q4_K") else None  # the capture is of the Q4_K kernel only
-            ent = json.load(open(tf)).get(key, {}) if key else {}
-            if ent.get("ratio"):
-                traffic, traffic_src = ent["ratio"] * alg_per_launch, ent.get("source")
-        except Exception:  # noqa: BLE001
-            traffic = None
     # HBM-write roofline (SURVEY.md §8(d)): bytes WRITTEN per launch against what a store-only kernel sustains on this box, measured now.
     # A probe failure must never fail the bench: the keys are null then.
     write_peak = copy_probe = None
@@ -701,7 +707,7 @@ def main():
                     "hbm_write_frac": ((part["out_bytes"] / max(n_launch, 1)) / (avg_launch_ms / 1e3) / 1e9 / write_peak) if write_peak and avg_launch_ms > 0 else None,
                     "hbm_write_note": "a device-resident bf16 copy reads what it writes: half its traffic is reads, so its write fraction is capped near 0.5 and the "
                                       ">= 0.70 HBM-write target only applies to expanding conversions (see `secondary`)" if spec["kind"] == "llama" else None,
-                    "traffic": traffic, "traffic_source": traffic_src, "peak_source": peak_src, "algorithmic_bytes_per_launch": alg_per_launch, "avg_launch_ms": avg_launch_ms,
+                    "peak_source": peak_src, "algorithmic_bytes_per_launch": alg_per_launch, "avg_launch_ms": avg_launch_ms,
                     "launches_per_step": n_launch,
                     "write_only_frac_of_peak": (part["out_bytes"] / max(n_launch, 1)) / (avg_launch_ms / 1e3) / 1e9 / peak if avg_launch_ms > 0 else 0.0}
     roofline = hbm_roofline
@@ -735,10 +741,10 @@ def main():
         pk_meas = probe_mean if probe_mean > 0 else None
         nvlink = {"bytes_per_step_per_gpu": moved, "stage_ms": stage_ms, "achieved_GBps_per_gpu": gbps, "peak_measured": pk_meas, "peak_measured_min_over_ranks": probe_min or None,
                   "peak_measured_how": "cudaMemcpyAsync D2D of 1 GiB from the ring neighbour's attached buffer, all ranks at once, best of 3, mean over ranks",
-                  "peak_nominal": 900.0, "frac_of_measured": gbps / pk_meas if pk_meas else None, "frac_of_nominal": gbps / 900.0, "form": form}
-        roofline = {"bound": "nvlink", "kernel": "kk_convert_kernel", "achieved": gbps, "peak": pk_meas or 900.0, "unit": "GB/s",
-                    "frac": gbps / (pk_meas or 900.0), "peak_source": "peer-copy probe measured in this run (see nvlink.peak_measured_how)" if pk_meas else "nominal 900 GB/s per direction (probe failed)",
-                    "peak_nominal": 900.0, "frac_of_nominal": gbps / 900.0, "traffic": None, "bytes_per_step_per_gpu": moved, "stage_ms": stage_ms, "form": form,
+                  "peak_nominal": H100_NVLINK_GBPS, "frac_of_measured": gbps / pk_meas if pk_meas else None, "frac_of_nominal": gbps / H100_NVLINK_GBPS, "form": form}
+        roofline = {"bound": "nvlink", "kernel": "kk_convert_kernel", "achieved": gbps, "peak": pk_meas or H100_NVLINK_GBPS, "unit": "GB/s",
+                    "frac": gbps / (pk_meas or H100_NVLINK_GBPS), "peak_source": "peer-copy probe measured in this run (see nvlink.peak_measured_how)" if pk_meas else "nominal 450 GB/s per direction (probe failed)",
+                    "peak_nominal": H100_NVLINK_GBPS, "frac_of_nominal": gbps / H100_NVLINK_GBPS, "bytes_per_step_per_gpu": moved, "stage_ms": stage_ms, "form": form,
                     "hbm_side": {k: hbm_roofline[k] for k in ("achieved", "peak", "frac", "algorithmic_bytes_per_launch", "avg_launch_ms", "launches_per_step")}}
 
     # ---- optional NCCL comparison collective ----------------------------------------------------------------
@@ -754,7 +760,7 @@ def main():
             ctx = cpu_port_setup(path, None if file_bytes <= (40 << 30) else 40 << 30)
             cpu_port_step(ctx)  # untimed: parallel first touch of the output buffer
             cpu_port_step(ctx)
-            ts = [cpu_port_step(ctx) for _ in range(5)]
+            ts = [cpu_port_step(ctx) for _ in range(args.steps)]
             cpu = {"value": ctx[3] / statistics.median(ts) / 1e9, "unit": UNIT, "cores": os.cpu_count() or 1, "kind": "port",
                    "sample": (("the whole checkpoint" if ctx[3] == file_bytes else f"first {ctx[3] / 1e9:.2f} GB of the checkpoint") +
                               f" ({ctx[3] / 1e9:.2f} GB), median of {len(ts)} passes after 2 untimed ones, pread + convert into host memory, all OpenMP threads"),
@@ -782,7 +788,7 @@ def main():
         "config": {"workload": spec["name"], "file_bytes": file_bytes, "tensors": len(ref.tensors), "shards": len(ref.shards),
                    "mode": {0: "single", 1: "broadcast (sharded ingest + fused P2P fan-out)",
                             2: "scatter" + (" (row-parallel tensors exchanged over NVLink: KK_LOAD_SCATTER_EXCHANGE)" if exchange else "")}[mode], "pool_bytes_per_gpu": pool_bytes,
-                   "l2": "inputs (>= 2 GB per GPU) far larger than the 126 MB L2; no flush needed", "files": f"warm in {os.path.dirname(d) or d}: written, then read twice by the ranks before anything is timed" + (", pages interleaved over the host's NUMA nodes (set_mempolicy while writing)" if _INTERLEAVED else ""),
+                   "l2": "inputs (>= 2 GB per GPU) far larger than the 50 MB L2; no flush needed", "files": f"warm in {os.path.dirname(d) or d}: written, then read twice by the ranks before anything is timed" + (", pages interleaved over the host's NUMA nodes (set_mempolicy while writing)" if _INTERLEAVED else ""),
                    "staging": "zero-copy pinned reads" if args.zerocopy else "pinned ring + H2D copy engine", "read_mode": os.environ.get("KUKEON_GPULOAD_READ", "auto (tmpfs shards: mapping + streaming stores + per-range MADV_DONTNEED; other file systems: pread)"), "verified_vs_files": verified,
                    **({"transpose_tiles": "8 source rows x <= 4 KiB, thread = column, 16-byte stores"} if spec["kind"] == "gpt2" else {})},
         "clocks": ck,
@@ -810,8 +816,7 @@ def main():
         line["raw_stages_ms_rank0"] = {"fanout_ms": sum(a for a, _ in raw_ms) / len(raw_ms), "convert_ms": sum(b for _, b in raw_ms) / len(raw_ms)}
     if world > 1 and mode == gpupool.MODE_BROADCAST:
         line["scaling_note"] = ("value(N) / (N x value(1)) is not a parallel efficiency here: at N = 1 a step is a copy inside one GPU's HBM, at N > 1 it is a "
-                                "broadcast whose floor is NVLink ingress, (N-1)/N x checkpoint bytes per GPU at the link rate — at most ~0.28 of N x value(1) "
-                                "for N = 8.  The per-N figure is roofline.frac (bound nvlink); end to end it is e2e.file_GBps and time_to_agent_ready_s.")
+                                "broadcast whose floor is NVLink ingress, (N-1)/N x checkpoint bytes per GPU at the link rate.  The per-N figure is roofline.frac (bound nvlink); end to end it is e2e.file_GBps and time_to_agent_ready_s.")
     if secondary is not None:
         line["secondary"] = secondary
     if secondary_g is not None:
@@ -882,6 +887,50 @@ def main():
         dist.destroy_process_group()
 
 
+def _f8e4m3_to_f32(b):
+    b = b.astype(np.int32)
+    e, mant = (b >> 3) & 15, (b & 7).astype(np.float32)
+    v = np.where(e == 0, mant / 8 * 2.0 ** -6, (1 + mant / 8) * np.exp2(e.astype(np.float32) - 7)).astype(np.float32)
+    v = np.where((e == 15) & (b & 7 == 7), np.float32(np.nan), v)
+    return np.where(b & 0x80, -v, v).astype(np.float32)
+
+
+# pool dtype -> (element bytes, decoder of the raw little-endian bytes): floats as float32 (F64 as float64), integers as float64 (exact for
+# every 8-32-bit value and for 64-bit values within +-2^53), FP8 decoded exactly; any other verbatim type as its raw bytes, one float64 each
+_DUMP_DECODE = {
+    "BF16": (2, lambda b: (b.view("<u2").astype(np.uint32) << 16).view(np.float32)),
+    "F16": (2, lambda b: b.view("<f2").astype(np.float32)), "F32": (4, lambda b: b.view("<f4").copy()), "F64": (8, lambda b: b.view("<f8").copy()),
+    "F8_E5M2": (1, lambda b: (b.astype(np.uint16) << 8).view(np.float16).astype(np.float32)), "F8_E4M3": (1, _f8e4m3_to_f32),
+    **{k: (np.dtype(t).itemsize, lambda b, t=t: b.view(t).astype(np.float64))
+       for k, t in (("BOOL", "u1"), ("U8", "u1"), ("I8", "i1"), ("U16", "<u2"), ("I16", "<i2"), ("U32", "<u4"), ("I32", "<i4"), ("U64", "<u8"), ("I64", "<i8"))},
+}
+
+
+def dump_outputs(m, ref, local: int, out_dir: str) -> None:
+    """What the last timed step left in this device's pool, as a caller reading it would receive it: one array per tensor (float32, or float64
+    where _DUMP_DECODE says so), written to out_dir/<tensor name>.npy.  A tensor is written whole when the per-tensor share of half of
+    DUMP_MAX_BYTES holds it; otherwise that share is taken as windows of consecutive elements at positions drawn from a generator seeded with
+    the tensor's index, so two builds given the same arguments dump the same elements."""
+    n_t = max(len(ref.tensors), 1)
+    per_tensor = (DUMP_MAX_BYTES // 2 - 256 * n_t) // 8 // n_t  # elements, at most 8 bytes each; 256 B per file for the .npy header
+    if per_tensor < 1:
+        raise SystemExit(f"--dump-outputs: {n_t} tensors do not fit {DUMP_MAX_BYTES >> 20} MiB")
+    os.makedirs(out_dir, exist_ok=True)
+    raw = (1, lambda b: b.astype(np.float64))
+    for i, r in enumerate(ref.tensors):
+        pl = m.placements(r["name"])[0]
+        es, decode = _DUMP_DECODE.get(pl.dtype, raw)
+        n = pl.nbytes // es
+        if n <= per_tensor:
+            out = decode(m.read(local, pl.pool_offset, n * es))
+            out = out.reshape(pl.shape) if int(np.prod(pl.shape)) == n else out
+        else:
+            win = min(1024, per_tensor)
+            starts = np.sort(np.random.default_rng(i).choice(n // win, per_tensor // win, replace=False)) * win
+            out = np.concatenate([decode(m.read(local, pl.pool_offset + int(s0) * es, win * es)) for s0 in starts])
+        np.save(os.path.join(out_dir, r["name"].replace("/", "_") + ".npy"), out)
+
+
 def args_for_secondary(args, workload="mixtral-q4k", layers=4):
     import copy
     a = copy.copy(args)
@@ -907,7 +956,7 @@ def secondary_kernel_stage(args, pool, gpupool, modelhub, peak, write_peak, work
             m.stage_resident()
             for _ in range(3):
                 m.convert_resident()
-            steps = 10
+            steps = args.steps
             runs = [m.convert_resident() for _ in range(steps)]
             part = m.stats()["parts"][0]
         finally:
@@ -935,8 +984,8 @@ def secondary_q4k(args, pool, gpupool, modelhub, peak, write_peak):
 
 
 def secondary_gpt2(args, pool, gpupool, modelhub, peak, write_peak):
-    """GPT-2-small f32 -> bf16 with the Conv1D weights transposed (BASELINE config 1's checkpoint, 0.5 GB; small: ~105 tiles per SM, so launch
-    ramp-up and tail are a visible part of its 0.15 ms)."""
+    """GPT-2-small f32 -> bf16 with the Conv1D weights transposed (BASELINE config 1's checkpoint, 0.5 GB; small: ~100 tiles per SM, so launch
+    ramp-up and tail are a visible part of its time)."""
     return secondary_kernel_stage(args, pool, gpupool, modelhub, peak, write_peak, "gpt2", 0, gpupool.LOAD_GPT2_CONV1D_T,
                                   "kernel stage only (resident image): BASELINE config 1's checkpoint, f32 -> bf16 casts + Conv1D transposes")
 

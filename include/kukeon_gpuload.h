@@ -1,5 +1,5 @@
 /*
- * kukeon_gpuload.h — C ABI of libkukeon_gpuload.so, the Blackwell-native model-hub weight loader.
+ * kukeon_gpuload.h — C ABI of libkukeon_gpuload.so, the model-hub weight loader for NVIDIA H100 (sm_90a).
  *
  * This is the drop-in boundary of the hot path named by BASELINE.json's north_star: kukeond keeps a Go
  * API (modelhub.Pull / Load / Mount, gpupool, the Cell hooks) and every one of those calls bottoms

@@ -1,4 +1,4 @@
-"""kukeon_b200 — Blackwell-native model-hub weight loader for kukeon.
+"""kukeon_b200 — H100-native (sm_90a) model-hub weight loader for kukeon (the package keeps its original name).
 
 The product is `libkukeon_gpuload.so` (C ABI in include/kukeon_gpuload.h, sources in kukeon_b200/csrc).
 `gpupool` is the ctypes binding (twin of the Go `internal/gpupool` cgo shim); `modelhub` mirrors the

@@ -401,8 +401,8 @@ int kk_checksum(kk_model* m, int device, uint64_t off, uint64_t nbytes, uint64_t
     if (off % 8) kk::fail(KK_EINVAL, "pool_offset must be a multiple of 8");
     kk::Device& d = m->ctx->devs[(size_t)m->dev_idx[(size_t)li]];
     KK_CUDA(cudaSetDevice(device));
-    // the accumulator lives in the device's scratch words: a cudaMalloc + cudaFree pair per call synchronises the whole device and measured
-    // 70-170 ms every few calls next to a 16 GB pool (profiles/r02/e2e_read_modes_q.jsonl)
+    // the accumulator lives in the device's scratch words: a cudaMalloc + cudaFree pair per call synchronises the whole device and, next to a
+    // 16 GB pool, stalls for tens of milliseconds every few calls
     std::lock_guard<std::mutex> one(*d.sum_mu);
     unsigned long long* acc = (unsigned long long*)(d.sched + 32);
     KK_CUDA(cudaMemsetAsync(acc, 0, 8, d.stream));

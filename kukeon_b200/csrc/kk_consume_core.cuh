@@ -47,7 +47,7 @@ KK_DQ_DEV void consume_f32(const Dsts& D, uint32_t pay, uint32_t n, uint64_t dst
   if ((pay & 15u) == 0) {
     // 4 elements per thread and step: one 16-byte load at a 16-byte lane stride (a warp reads 512 contiguous bytes: 4 wavefronts, the minimum)
     // and one 8-byte store (a warp writes 256 contiguous bytes).  Round 1 took 8 elements per thread — two 16-byte loads at a 32-byte lane
-    // stride, a 2-way bank conflict on each (1.23 M excessive wavefronts in the GPT-2 load, profiles/r02/prof_gpt2: all of them here).
+    // stride, a 2-way bank conflict on each.
     const uint32_t nq = n >> 2;
     for (uint32_t g = ctid; g < nq; g += kConsumerThreads) {
       const uint4 a = lds128(pay + (g << 4));
@@ -107,7 +107,7 @@ KK_DQ_DEV void consume_f16(const Dsts& D, uint32_t pay, uint32_t n, uint64_t dst
 // dependency chains are independent and fully unrolled (ILP hides the ALU latency with only 2 warps/SMSP).
 // Expansion of one quad.  FAST: c = -(d*sc) * 2^23 (exact: a power-of-two scaling) lets ONE FMA turn the magic-number float 2^23 + q straight
 // into the rounded product — fma(dsc, 2^23 + q, c) = round(dsc * q), the same single rounding as __fmul_rn(dsc, (float)q) — instead of
-// FADD + FMUL per element (the loop is issue-bound: 70 % issue-active at 0.87 of the copy peak, profiles/r02/prof_Q4_K).  The identity
+// FADD + FMUL per element (the loop is issue-bound).  The identity
 // holds bit for bit only for a finite scale that is not negative: with +-inf the FMA sees inf - inf (NaN, where the two-step form gives
 // +-inf for q > 0), and for q = 0 under a negative scale it yields +0 where the product is -0 (visible when the sub-block minimum is 0).
 // Real checkpoints have d >= 0 and finite — every quad takes the fast form — but random bytes are part of the parity tests, so the warp
@@ -199,7 +199,7 @@ KK_DQ_DEV void consume_q4k(const Dsts& D, uint32_t pay, uint32_t nblk, uint64_t 
     else q4k_quad<false, false>(D, pay, b0, nb, dst_off, lane);
   }
 }
-// Q5_K through the same quads (round 1 gave it one block per warp iteration with ten shared loads per lane: 0.74 of the copy peak, the slowest
+// Q5_K through the same quads (round 1 gave it one block per warp iteration with ten shared loads per lane, the slowest
 // dequantiser; the header decode is now amortised over four blocks and handed out by shuffles like Q4_K's)
 KK_DQ_DEV void consume_q5k(const Dsts& D, uint32_t pay, uint32_t nblk, uint64_t dst_off, int cwarp, int lane) {
   const bool al = (pay & 15u) == 0;  // 176-byte blocks keep the tile's alignment class

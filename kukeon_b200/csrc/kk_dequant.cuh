@@ -55,7 +55,7 @@ KK_DQ_DEV uint32_t lds32_funnel(uint32_t a) {
 // lds32_any is one load.  Every other size takes the funnel: branch-free, so all of a block's loads issue back to back.  (Round 1 kept the
 // branchy form for the 256-weight blocks of 4k + 2 bytes — their alignment is warp-uniform, so it costs no divergence and one
 // instruction less on average — but each of its four loads sat in its own BSSY / BRA / BSYNC region and exposed its shared-memory latency
-// separately; measured on hardware that put Q3_K at 0.54 of the copy peak, TQ1_0 and IQ2_XXS at 0.70.)
+// separately, which left Q3_K, TQ1_0 and IQ2_XXS latency-bound.)
 template <uint32_t BLOCK_BYTES>
 KK_DQ_DEV uint32_t lds32_blk(uint32_t a) { return (BLOCK_BYTES % 4u != 0u) ? lds32_funnel(a) : lds32_any(a); }
 // Eight payload bytes at ANY address a -> two words: the three aligned words that cover them, funnel-shifted into place (SHF.R.W).
@@ -190,7 +190,7 @@ KK_DQ_DEV void consume_legacy32(const Dsts& D, uint32_t pay, uint32_t nblk, uint
 KK_DQ_DEV void consume_q2k(const Dsts& D, uint32_t pay, uint32_t nblk, uint64_t dst_off, int cwarp, int lane) {
   const uint32_t q_off = 16u + 32u * (uint32_t)(lane >> 4) + 8u * (uint32_t)(lane & 3);
   const uint32_t sh = 2u * (uint32_t)((lane >> 2) & 3);
-  // (no `#pragma unroll 2` here: measured slower with it on a B200, profiles/r02/types_roofline_{a,b}.json — this loop was not latency-bound)
+  // (no `#pragma unroll 2` here: this loop is not latency-bound, and it ran slower unrolled)
   for (uint32_t b = (uint32_t)cwarp; b < nblk; b += kConsumerWarps) {
     const uint32_t blk = pay + b * KK_Q2K_BLOCK_BYTES;
     const float d = lds_f16(blk + 80u), dmin = lds_f16(blk + 82u);
@@ -462,7 +462,7 @@ KK_DQ_DEV void consume_iq2xs(const Dsts& D, uint32_t pay, uint32_t nblk, uint64_
 // IQ2_S (82 B): d f16 | qs[32] | signs[32] | qh[8] (2 more index bits per entry) | scales[8]
 KK_DQ_DEV void consume_iq2s(const Dsts& D, uint32_t pay, uint32_t nblk, uint64_t dst_off, int cwarp, int lane) {
   const uint32_t l = (uint32_t)lane;
-  // (no `#pragma unroll 2` here: measured slower with it on a B200, profiles/r02/types_roofline_{a,b}.json — this loop was not latency-bound)
+  // (no `#pragma unroll 2` here: this loop is not latency-bound, and it ran slower unrolled)
   for (uint32_t b = (uint32_t)cwarp; b < nblk; b += kConsumerWarps) {
     const uint32_t blk = pay + b * KK_IQ2S_BLOCK_BYTES;
     const float d = lds_f16(blk);

@@ -1,4 +1,4 @@
-// sm_100a kernels of the weight loader: one persistent, warp-specialised convert / fan-out kernel
+// sm_90a kernels of the weight loader: one persistent, warp-specialised convert / fan-out kernel
 // plus a checksum kernel.  No tensor cores — the path has no contraction; it is HBM / NVLink bound.
 //
 // kk_convert_kernel:
@@ -28,7 +28,7 @@ namespace kk {
 namespace {
 
 constexpr int kStages = 4;
-constexpr int kConsumerWarps = 16;  // 16 rather than 8: +4 % on q4_K, 1.7x on the transposes; 20 (80 registers) measured no faster (profiles/r02)
+constexpr int kConsumerWarps = 16;  // 16 rather than 8: faster q4_K and much faster transposes; 20 (80 registers) is no faster
 constexpr int kConsumerThreads = kConsumerWarps * 32;
 constexpr int kThreads = 32 + kConsumerThreads;  // 544
 constexpr uint32_t kStageBytes = KK_TILE_SRC_BYTES + KK_STAGE_PAD;
@@ -244,8 +244,8 @@ __device__ __forceinline__ KKSeg load_seg(const KKSeg* p) {
 }
 
 // DYN: tiles after the first are drawn from L.sched (see the producer); !DYN: static round-robin, the consumers count their tiles themselves —
-// exactly the round-1 loops.  Two instantiations rather than a run-time switch: with the switch the STATIC path of the transposing load measured
-// 0.161 ms where the dedicated loops take 0.148 ms (same box, libraries built from the commits in between: profiles/r02/gpu_call_m.log).
+// exactly the round-1 loops.  Two instantiations rather than a run-time switch: with the switch the STATIC path of the transposing load ran
+// slower than the dedicated loops.
 template <bool DYN>
 __global__ void __launch_bounds__(kThreads, 1) kk_convert_kernel(const ConvertLaunch L) {
   extern __shared__ __align__(128) uint8_t smem[];
@@ -271,10 +271,9 @@ __global__ void __launch_bounds__(kThreads, 1) kk_convert_kernel(const ConvertLa
     // ===== producer =====
     if (lane == 0) {
       // Tile scheduling.  Static round-robin (tile = blockIdx.x + k * gridDim.x) leaves the SMs unevenly loaded although every CTA gets the same
-      // number of tiles: ncu showed sm__cycles_active at 0.86 of the kernel's duration for Q4_K and 0.92 for the bf16 copy, the fastest SM done
-      // at 0.80 — SMs do not all see the same memory (two dies, their own HBM stacks), and the kernel ends with the slowest CTA.  So after its
-      // first, static tile a CTA draws batches of kBatch tiles from a global counter; the draw for batch b + 1 is issued while batch b is being
-      // produced, so the atomic's round trip is off the critical path even for the copy op (0.75 us per tile).
+      // number of tiles: SMs do not all see the same memory at the same cost (L2 partitions, HBM stacks), and the kernel ends with the slowest
+      // CTA.  So after its first, static tile a CTA draws batches of kBatch tiles from a global counter; the draw for batch b + 1 is issued while
+      // batch b is being produced, so the atomic's round trip is off the critical path even for the copy op.
       constexpr uint32_t kBatch = 2;
       uint32_t cur = 0;
       KKSeg seg = load_seg(L.segs);

@@ -1,4 +1,4 @@
-// Launch interface of the sm_100a kernels (implemented in kk_kernels.cu).
+// Launch interface of the sm_90a kernels (implemented in kk_kernels.cu).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -180,21 +180,19 @@ struct DevScratch {
   }
 };
 
-// How a chunk's long contiguous ranges travel from the page cache into the pinned slot.  Measured on the B200 box, Llama-3-8B (16 GB) from tmpfs,
-// 16 reader threads (profiles/r02/e2e_read_modes_{o,p,q}.jsonl):
-//   pread                       the kernel's copy_to_user: 0.31-0.33 s of copying per thread, the load is reader-bound at 0.33-0.34 s (47-49 GB/s)
+// How a chunk's long contiguous ranges travel from the page cache into the pinned slot (Llama-3-8B from tmpfs, 16 reader threads):
+//   pread                       the kernel's copy_to_user, 4 KiB at a time: the load is reader-bound
 //   mapping + memcpy            no faster than pread, and the final munmap of a checkpoint-sized mapping is ONE thread tearing down 4 M page-table
-//                               entries: + 0.33 s per load
-//   mapping + streaming stores  0.17-0.19 s per thread (no read-for-ownership of the slot's lines, which only the DMA engine reads next) — with the
-//                               same munmap bill
+//                               entries
+//   mapping + streaming stores  about half pread's copy time per thread (no read-for-ownership of the slot's lines, which only the DMA engine
+//                               reads next) — with the same munmap bill
 //   ... + MADV_DONTNEED of each range right after its copy (the reader threads drop their own page-table entries in parallel, the final munmap
-//                               finds none: 1 ms): the load becomes H2D-bound, 0.303-0.307 s = 52.5 GB/s = 0.96 of the pinned-H2D probe.  DEFAULT for
-//                               shards on tmpfs; other file systems keep pread (a mapping of a cold file would fault page by page into the disk).
-//   MAP_POPULATE mapping per range: 0.9 s per thread (every mmap / munmap takes the process's mm lock exclusively).
+//                               finds none): the load becomes H2D-bound.  DEFAULT for shards on tmpfs; other file systems keep pread (a mapping of
+//                               a cold file would fault page by page into the disk).
+//   MAP_POPULATE mapping per range: slower than pread (every mmap / munmap takes the process's mm lock exclusively).
 //   cache-resident bounce ring (4 x 256 KiB pinned pieces per reader between mapping and device slot, so that neither the CPU's stores nor the copy
-//                               engine's reads reach DRAM): CPU copy 2x faster again, but 64 K small H2D copies starve the copy engines — 2 GPUs on one
-//                               socket 288.6 -> 382.2 ms per step (profiles/r02/gpu_call_w.log).
-// The measured losers are deleted (git history: ed69c4b..50a97f8 carry them); what is left is the default and one switch:
+//                               engine's reads reach DRAM): faster CPU copy, but 64 K small H2D copies starve the copy engines.
+// The slower forms are deleted (git history: ed69c4b..50a97f8 carry them); what is left is the default and one switch:
 // KUKEON_GPULOAD_READ = pread (never map) | mapped (map every shard, whatever the file system).  Measurement knob, not API.
 enum ReadMode { kReadAuto = 0, kReadPread, kReadMapped };
 ReadMode read_mode() {
@@ -255,7 +253,7 @@ void read_chunk(const Chunk& c, const FdSet& fds, const Index& ix, uint8_t* pinn
       continue;
     }
     // short ranges (column-slice rows of a SCATTER load: thousands of 2-7 KB runs per chunk) stay on pread: copied out of the mapping the 70B
-    // scatter load measured 1.99 s against 1.51 s — a first-touch page fault per row costs more than the syscall (round 1, 8 x B200)
+    // scatter load is slower — a first-touch page fault per row costs more than the syscall
     pread_full(fds.fds[c.shard], pinned + r.buf_off, r.len, r.file_off, ix.shards[c.shard]);
   }
 }
@@ -371,9 +369,9 @@ void fill_dsts(kk_model* m, int li, ConvertLaunch& L) {
   pad_dsts_for_test(L);
 }
 
-// Tile scheduling of a launch: dynamic (counters of the launching stream) except for transposing loads.  Their 16-byte column stores fill a
-// 32-byte sector only together with the neighbouring row group's tile, and under static round-robin those two tiles run at about the same time
-// on different SMs and meet in L2; with dynamic draws GPT-2-small measured 0.173 ms against 0.146 ms static (profiles/r02/gpt2_quick_{e,h}.json).
+// Tile scheduling of a launch: dynamic (counters of the launching stream) for every plan.  On H100 this includes the transposing loads: the
+// GPT-2-small load takes 0.51 ms with dynamic draws against 0.70 ms under static round-robin (one H100 SXM, 700 W limit, 50 launches each,
+// twice, same build).
 uint32_t* sched_for(const kk_model* m, uint32_t* stream_counters) {
   // measurement knob (A/B of the two schedulers on one box; not part of the API): KUKEON_GPULOAD_SCHED=static | dynamic forces one
   static const int forced = [] {
@@ -382,7 +380,8 @@ uint32_t* sched_for(const kk_model* m, uint32_t* stream_counters) {
   }();
   if (forced == 1) return nullptr;
   if (forced == 2) return stream_counters;
-  return (m->plan.flags & KK_LOAD_GPT2_CONV1D_T) ? nullptr : stream_counters;
+  (void)m;
+  return stream_counters;
 }
 
 // Ingest plan part `part` on local device `li`.
@@ -777,7 +776,7 @@ kk_ctx* ctx_open(const kk_config& cfg_in) {
     fail(KK_ECUDA, "no usable CUDA device (%s); this library has no CPU path", e == cudaSuccess ? "device count is 0" : cudaGetErrorString(e));
   for (int i = 0; i < cfg.n_devices; ++i)
     if (cfg.devices[i] < 0 || cfg.devices[i] >= count) fail(KK_EINVAL, "device ordinal %d not present (%d devices)", cfg.devices[i], count);
-  if (cfg.n_reader_threads == 0) cfg.n_reader_threads = 16;  // 16 x ~4 GB/s of page-cache pread saturates a Gen5 x16 link (profiles/r01)
+  if (cfg.n_reader_threads == 0) cfg.n_reader_threads = 16;  // 16 x ~4 GB/s of page-cache pread saturates a Gen5 x16 link
   if (cfg.n_staging_buffers == 0) cfg.n_staging_buffers = 2 * cfg.n_reader_threads;
   if (cfg.n_reader_threads > 64) fail(KK_EINVAL, "n_reader_threads %u too large", cfg.n_reader_threads);
   if (cfg.n_staging_buffers < cfg.n_reader_threads) cfg.n_staging_buffers = cfg.n_reader_threads;
@@ -790,7 +789,7 @@ kk_ctx* ctx_open(const kk_config& cfg_in) {
   c->devs.resize((size_t)cfg.n_devices);
   try {
     // One thread per device, all at once: the pinned ring (cudaHostAlloc pins and maps 0.5 GiB per device by default) dominates kk_open, and eight
-    // devices set up one after the other cost 4.7 s in the one-process shape (profiles/r02/bench_n8_head.json: single_process.kk_open_s).  Each
+    // devices set up one after the other add up to seconds in the one-process shape.  Each
     // thread is bound to its device's NUMA node, so the slots are first-touched / pinned there.
     std::vector<std::exception_ptr> errs((size_t)cfg.n_devices);
     std::vector<std::thread> setup;
@@ -802,7 +801,9 @@ kk_ctx* ctx_open(const kk_config& cfg_in) {
           KK_CUDA(cudaSetDevice(d.ordinal));
           cudaDeviceProp prop;
           KK_CUDA(cudaGetDeviceProperties(&prop, d.ordinal));
-          if (prop.major < 10) fail(KK_EUNSUPPORTED, "device %d is sm_%d%d; this build carries sm_100a code only", d.ordinal, prop.major, prop.minor);
+          // the library carries sm_90a SASS and no PTX: arch-specific code loads on compute capability 9.0 only
+          if (prop.major != 9 || prop.minor != 0)
+            fail(KK_EUNSUPPORTED, "device %d is sm_%d%d; this build carries sm_90a code only", d.ordinal, prop.major, prop.minor);
           d.sm_count = prop.multiProcessorCount;
           KK_CUDA(kernels_init_device());
           d.kernels_ready = true;
@@ -1076,9 +1077,8 @@ kk_model* model_load(kk_ctx* c, const std::string& path, const kk_load_opts& opt
       m->slice_base = mine.first & ~(uint64_t)255;
       const uint64_t sb = mine.second > m->slice_base ? mine.second - m->slice_base : 0;
       KK_CUDA(cudaSetDevice(c->devs[(size_t)m->dev_idx[0]].ordinal));
-      // whole 2 MiB multiples, like the pools: cudaIpcOpenMemHandle of such an allocation is ~50x cheaper than of one the driver carved out of
-      // shared blocks (measured at N = 8: seven 16 GB pools map in 0.07 s, seven 2 GB slice buffers of odd size took 0.66 s — and in round 1,
-      // before the pools were rounded, seven pools took 3.6 s; profiles/r02/bench_n8_*.json)
+      // whole 2 MiB multiples, like the pools: cudaIpcOpenMemHandle of such an allocation is far cheaper than of one the driver carved out of
+      // shared blocks (at N = 8, seven rounded 16 GB pools map faster than seven 2 GB slice buffers of odd size)
       cudaError_t se = cudaMalloc((void**)&m->slice_buf, align_up(sb ? sb : 256, 2u << 20));
       if (se != cudaSuccess) { cudaGetLastError(); m->slice_buf = nullptr; fail(KK_ENOMEM, "cudaMalloc(%llu) for the slice buffer failed", (unsigned long long)sb); }
     }

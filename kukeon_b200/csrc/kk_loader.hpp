@@ -77,7 +77,7 @@ struct kk_model {
   std::vector<uint64_t> pool_bytes;  // per local device
   // What kk_export hands out is fixed once the pools exist: the manifest text and the pool's CUDA IPC handle are built on first use and kept.  Every
   // cell that mounts the model exports again, and the calls underneath (cudaIpcGetMemHandle, cudaGetDeviceProperties) go through the driver's
-  // system-wide lock: 2.5 ms normally, 11-144 ms when another process on the host holds it (profiles/r02/gpu_call_u.log).
+  // system-wide lock, where they wait behind whatever another process on the host is doing in the driver.
   std::mutex export_mu;
   std::vector<std::string> manifest_cache;               // per local device, empty = not built yet
   std::vector<std::vector<uint8_t>> pool_handle_cache;   // per local device, empty = not asked yet

@@ -8,10 +8,9 @@
 #define KK_STAGE_PAD 128u        /* slack so a 16-B-aligned superset of a misaligned tile still fits */
 #define KK_Q4K_BLOCK_BYTES 144u
 #define KK_Q4K_BLOCK_ELEMS 256u
-#define KK_Q4K_TILE_BLOCKS 224u  /* 224*144 = 32256 B in, 224*512 = 114688 B out.  16 consumer warps x 4 blocks = 64 blocks per sweep, so 3.5 sweeps; measured
-                                    against 192-block tiles (3 full sweeps), contiguous 14-block runs per warp, a rotated warp order and 20 warps
-                                    (profiles/r02/q4k_ab_*.json): all within 2 % and none faster, so the simplest form stays.  Swept again under dynamic tile
-                                    scheduling (186 / 200 / 208 / 216 / 221 / 223 blocks, profiles/r02/q4k_tile_sweep_h.txt): 1.642 - 1.671 ms against 1.651 */
+#define KK_Q4K_TILE_BLOCKS 224u  /* 224*144 = 32256 B in, 224*512 = 114688 B out.  16 consumer warps x 4 blocks = 64 blocks per sweep, so 3.5 sweeps; timed
+                                    against 192-block tiles (3 full sweeps), contiguous 14-block runs per warp, a rotated warp order, 20 warps and, under
+                                    dynamic tile scheduling, 186-223 blocks: none faster, so the simplest form stays */
 #define KK_Q8_0_BLOCK_BYTES 34u
 #define KK_Q8_0_BLOCK_ELEMS 32u
 #define KK_Q8_0_TILE_BLOCKS 960u /* 960*34 = 32640 B in (a multiple of 16), 960*64 = 61440 B out */
@@ -62,10 +61,10 @@
 #define KK_NVFP4_TILE_BLOCKS 908u /* 32688 B in */
 /* 2-D transposes (GPT-2 Conv1D): a tile is 8 source rows x up to KK_T_ROW_BYTES of each.  Eight bulk copies bring in a full 32 KiB stage (ONE when the
  * tile spans whole rows, which are then contiguous in the source); consumers read along rows — conflict-free at any pitch — and every thread packs
- * the 8 rows of one column into a single 16-byte store.  Measured on GPT-2-small against 32x128 tiles (0.36 of the copy peak) and 32-row x 960-byte
- * wide-store tiles (0.58): 0.80 (profiles/r02/t8_ab_*.json) — the other two geometries are gone. */
-#define KK_T_ROWS 8u             /* a multiple of 8; 16 x 2 KiB and 32 x 1 KiB tiles (whole-sector stores per thread) measured SLOWER: 0.195 / 0.211 ms */
-#define KK_T_ROW_BYTES 4096u     /* against 0.160 ms on GPT-2-small, profiles/r02/gpu_call_l.log.  Per staged row: 1024 32-bit or 2048 16-bit columns */
+ * the 8 rows of one column into a single 16-byte store.  Timed on GPT-2-small against 32x128 tiles and 32-row x 960-byte wide-store tiles, both
+ * slower — the other two geometries are gone. */
+#define KK_T_ROWS 8u             /* a multiple of 8; 16 x 2 KiB and 32 x 1 KiB tiles (whole-sector stores per thread) are slower on GPT-2-small */
+#define KK_T_ROW_BYTES 4096u     /* per staged row: 1024 32-bit or 2048 16-bit columns */
 #define KK_MAX_DST 8
 /* ConvertLaunch::flags */
 #define KK_LAUNCH_NO_BULK_STORE 0x1u  /* force the register path for aligned copies (A/B measurement) */

@@ -229,6 +229,23 @@ def forget_pool(model) -> None:
         del _POOL_SUMS[k]
 
 
+_SUN_PATH_MAX = 107  # sockaddr_un.sun_path holds 108 bytes including the terminating NUL
+
+
+def _unix_call(op, path: str) -> None:
+    """op(address) for the Unix socket at `path` (bind or connect).  A staged path can be longer than sun_path (cells live deep under the
+    daemon's run path): then the address is the socket's name inside an O_PATH descriptor of its directory, /proc/self/fd/<n>/<name>,
+    which the kernel resolves to the same file."""
+    if len(os.fsencode(path)) <= _SUN_PATH_MAX:
+        op(path)
+        return
+    d = os.open(os.path.dirname(path) or ".", os.O_PATH | os.O_DIRECTORY)
+    try:
+        op(f"/proc/self/fd/{d}/{os.path.basename(path)}")
+    finally:
+        os.close(d)
+
+
 class PoolFdServer(threading.Thread):
     """Hands the file descriptor of a VMM pool to whoever connects to `path` (a Unix socket staged in the directory that is bind-mounted
     read-only into the agent container — like a docker.sock, the socket stays connectable through the mount).  One message per connection:
@@ -244,7 +261,7 @@ class PoolFdServer(threading.Thread):
         except FileNotFoundError:
             pass
         self.sock = socket.socket(socket.AF_UNIX, socket.SOCK_STREAM)
-        self.sock.bind(path)
+        _unix_call(self.sock.bind, path)
         os.chmod(path, 0o660)
         self.sock.listen(16)
         self.sock.settimeout(0.2)
@@ -293,7 +310,7 @@ def unmount(spec: MountSpec) -> None:
 def receive_pool_fd(sock_path: str) -> tuple:
     """Agent side: connect to the staged socket, returns (fd, mapped_bytes).  The caller maps it with gpupool.ImportedPool and closes the fd."""
     with socket.socket(socket.AF_UNIX, socket.SOCK_STREAM) as c:
-        c.connect(sock_path)
+        _unix_call(c.connect, sock_path)
         msg, fds, _, _ = socket.recv_fds(c, 8, 1)
         if len(msg) != 8 or len(fds) != 1:
             raise OSError("pool fd server sent no descriptor")

@@ -10,10 +10,10 @@ from tools import sass_budget
 
 pytestmark = pytest.mark.skipif(shutil.which("nvcc") is None or shutil.which("nvdisasm") is None, reason="needs the CUDA toolkit (nvcc, nvdisasm)")
 
-# hot-path warp instructions per ONE-block-group of work (one destination pool, aligned loads) as committed in profiles/r01/sass_budget.md, + ~5 %; the
-# loops are unrolled twice since round 2 (two independent chains per iteration), which tools/sass_budget.py folds into its bytes-per-iteration table —
+# hot-path warp instructions per ONE-block-group of work (one destination pool, aligned loads) of the loops before they were unrolled, + ~5 %; the
+# loops are unrolled twice now (two independent chains per iteration), which tools/sass_budget.py folds into its bytes-per-iteration table —
 # so the comparison is made per KiB of algorithmic traffic, the quantity the issue ceiling is computed from
-# Q4_K / Q5_K: per four-block quad on the FMA form (round 2: 238 / 274; round 1 had 260 for Q4_K and 91 per single Q5_K block)
+# Q4_K / Q5_K: per four-block quad on the FMA form
 HOT_MAX = {
     "KK_OP_COPY": 42, "KK_OP_F32_BF16": 84, "KK_OP_F16_BF16": 60, "KK_OP_F8E4M3_BF16": 53, "KK_OP_F8E5M2_BF16": 53,
     "KK_OP_Q4K_BF16": 250, "KK_OP_Q8_0_BF16": 67, "KK_OP_Q6K_BF16": 88, "KK_OP_Q4_0_BF16": 68, "KK_OP_Q4_1_BF16": 80, "KK_OP_Q5_0_BF16": 85,

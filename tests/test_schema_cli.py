@@ -195,7 +195,7 @@ def test_merge_mounts_deduplicates_device_nodes(tmp_path):
     proc = tmp_path / "proc"
     for bus, minor in (("0000:1b:00.0", 1), ("0000:1c:00.0", 0)):
         os.makedirs(proc / bus)
-        (proc / bus / "information").write_text(f"Model: \t\t NVIDIA B200\nIRQ:   \t\t 16\nGPU UUID: \t GPU-x\nBus Location: \t {bus}\nDevice Minor: \t {minor}\n")
+        (proc / bus / "information").write_text(f"Model: \t\t NVIDIA H100 80GB HBM3\nIRQ:   \t\t 16\nGPU UUID: \t GPU-x\nBus Location: \t {bus}\nDevice Minor: \t {minor}\n")
     minor_of = lambda bus: modelhub.device_minor(bus, proc_root=str(proc))  # noqa: E731
     assert minor_of("0000:1B:00.0") == 1
     with pytest.raises(OSError):
@@ -208,3 +208,28 @@ def test_merge_mounts_deduplicates_device_nodes(tmp_path):
     merged = modelhub.merge_mounts([a, b, c])
     assert [d["path"] for d in merged.devices] == ["/dev/nvidiactl", "/dev/nvidia-uvm", "/dev/nvidia1", "/dev/nvidia0"]
     assert len(merged.device_cgroup) == 4 and all(r["allow"] and r["access"] == "rw" for r in merged.device_cgroup)
+
+
+def test_pool_fd_socket_works_beyond_the_unix_path_limit(tmp_path):
+    """A cell's staged directory can lie deeper than sockaddr_un's 108 bytes: the fd server still binds there and the agent side connects."""
+    from kukeon_b200 import modelhub
+
+    class _Model:
+        def export_fd(self, device):
+            r, w = os.pipe()
+            os.close(w)
+            return r, 4096
+
+    d = tmp_path.joinpath(*(["cell-directory-name"] * 8))
+    d.mkdir(parents=True)
+    path = str(d / "pool.sock")
+    assert len(path) > 108
+    srv = modelhub.PoolFdServer(_Model(), 0, path)
+    srv.start()
+    try:
+        fd, size = modelhub.receive_pool_fd(path)
+        os.close(fd)
+        assert size == 4096 and srv.served == 1
+    finally:
+        srv.stop()
+    assert not os.path.exists(path)

@@ -31,9 +31,9 @@ def main():
     pk = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(pk):
         peak = json.load(open(pk)).get("hbm_gbs")
-    # static prediction committed next to the profiles (tools/sass_budget.py --json): hot-path instructions -> issue ceiling per op
+    # static prediction (tools/sass_budget.py --json, when written next to this tool): hot-path instructions -> issue ceiling per op
     pred = {}
-    pj = os.path.join(ROOT, "profiles", "r01", "sass_budget.json")
+    pj = os.path.join(ROOT, "tools", "sass_budget.json")
     if os.path.exists(pj):
         pred = json.load(open(pj)).get("ops", {})
     opname = lambda dt: "KK_OP_" + dt.replace("_K", "K").replace("IQ4_NL", "IQ4NL").replace("IQ4_XS", "IQ4XS").replace("IQ2_XXS", "IQ2XXS").replace("IQ2_XS", "IQ2XS") \
@@ -65,7 +65,7 @@ def main():
                     if peak:
                         row["frac_of_copy_peak"] = row["GBps"] / peak
                     pr = pred.get(opname(dt))
-                    if pr:  # fraction of the issue slots the measured rate would need if only the hot path issued (Q4_K calibrates: 0.50 predicted, 0.62 measured)
+                    if pr:  # fraction of the issue slots the measured rate would need if only the hot path issued
                         row["predicted_issue_ceiling_GBps"] = pr["issue_ceiling_GBps"]
                         row["issue_fraction_at_measured_rate"] = row["GBps"] / pr["issue_ceiling_GBps"]
                     out["types"][dt] = row

@@ -5,13 +5,12 @@ dispatch line they were inlined at (`nvdisasm -gi`, built with -lineinfo), finds
 the op's main loop: warp instructions per iteration, the opcode mix, and — with the bytes one warp iteration reads and writes — warp
 instructions per KiB of algorithmic HBM traffic.  Put against the issue rate of the machine (4 schedulers x 1 warp instruction per clock per
 SM) this gives the traffic rate at which the loop would saturate instruction issue: a loop whose ceiling is below the HBM roofline is
-issue-bound however well the memory side is arranged.  Q4_K is the calibration point: measured 0.879 of the copy peak at 62 % issue-active
-(profiles/r01/prof_q4k_v2.*).
+issue-bound however well the memory side is arranged.
 
 A static count is an upper estimate of what issues (predicated-off instructions count; code behind a forward branch that is not taken
 counts) and knows nothing about stalls; it ranks the loops and says where the PRMT/FADD rewrites landed, it is not a measurement.
 
-    python tools/sass_budget.py [--md profiles/r01/sass_budget.md]
+    python tools/sass_budget.py [--md sass_budget.md] [--json sass_budget.json]
 """
 import argparse
 import collections
@@ -25,8 +24,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "kukeon_b200", "csrc")
 KERNEL_CU = os.path.join(CSRC, "kk_kernels.cu")
 
-SM_COUNT, SM_GHZ, ISSUE_PER_CLK = 148, 1.965, 4  # B200: 148 SMs, clocks sampled under load (profiles/README.md), 4 warp schedulers per SM
-HBM_PEAK_GBS = 6574.1                            # MEASURED_PEAKS.json hbm_gbs of round 1
+SM_COUNT, SM_GHZ, ISSUE_PER_CLK = 132, 1.98, 4  # H100 SXM: 132 SMs, 1980 MHz sampled during bench.py's timed steps (700 W limit), 4 warp schedulers per SM
+HBM_PEAK_GBS = 3350.0                           # H100 SXM data sheet (HBM3); the store-only probe measured 3,165 GB/s on the same card
 
 # bytes one WARP iteration of the op's main loop reads from the stage and writes to one pool: (in, out).  From the lane mappings in
 # kk_consume_core.cuh / kk_dequant.cuh: the 256-weight types take one block per warp iteration, the 32-weight types eight, Q4_K four
@@ -68,7 +67,7 @@ def disassemble(obj=None):
         obj = obj or fresh_object()
         if obj is None:
             obj = os.path.join(d, "k.o")
-            subprocess.check_call(["nvcc", "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo", "-I" + os.path.join(ROOT, "include"),
+            subprocess.check_call(["nvcc", "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo", "-I" + os.path.join(ROOT, "include"),
                                    "-c", KERNEL_CU, "-o", obj], cwd=CSRC, stderr=subprocess.DEVNULL)
         subprocess.check_call(["cuobjdump", "-xelf", "all", obj], cwd=d, stdout=subprocess.DEVNULL)
         cubin = [f for f in os.listdir(d) if f.endswith(".cubin")][0]
