@@ -168,7 +168,7 @@ int kk_peer_attach(kk_model* m, int rank, const void* h) {
   return guard([&] {
     need(m, "model");
     need(h, "ipc_handle");
-    kk::model_peer_attach(m, rank, h);
+    kk::model_peer_attach(m, kk::kPeerPool, rank, h, true);
   });
 }
 
@@ -179,19 +179,33 @@ int kk_peer_detach_all(kk_model* m) {
   });
 }
 
+// KK_BUF_* -> the peer buffer it names and whether its handle is a device pointer rather than a CUDA IPC handle; false for an unknown kind.
+static bool buf_kind(int which, kk::PeerKind& kind, bool& by_ptr) {
+  by_ptr = which == KK_BUF_POOL_PTR || which == KK_BUF_SLICE_PTR;
+  switch (which) {
+    case KK_BUF_POOL: case KK_BUF_POOL_PTR: kind = kk::kPeerPool; return true;
+    case KK_BUF_RAW: kind = kk::kPeerRaw; return true;
+    case KK_BUF_SLICE: case KK_BUF_SLICE_PTR: kind = kk::kPeerSlice; return true;
+  }
+  return false;
+}
+
 int kk_export_buffer(kk_model* m, int device, int which, void* h) {
   return guard([&] {
     need(m, "model");
     need(h, "ipc_handle");
     int li = kk::model_local_device(m, device);
-    if (which == KK_BUF_POOL) {
+    kk::PeerKind kind;
+    bool by_ptr;
+    if (!buf_kind(which, kind, by_ptr) || (kind == kk::kPeerPool && by_ptr)) kk::fail(KK_EINVAL, "unknown buffer kind %d", which);
+    if (kind == kk::kPeerPool) {
       if (m->nvls) kk::fail(KK_EUNSUPPORTED, "pools of a KK_FANOUT_NVLS model cannot be exported over CUDA IPC");
       kk::model_pool_ipc_handle(m, li, h);
-    } else if (which == KK_BUF_RAW) {
+    } else if (kind == kk::kPeerRaw) {
       kk::model_export_raw(m, li, h);
-    } else if (which == KK_BUF_SLICE || which == KK_BUF_SLICE_PTR) {
-      kk::model_export_slice(m, h, which == KK_BUF_SLICE_PTR);
-    } else kk::fail(KK_EINVAL, "unknown buffer kind %d", which);
+    } else {
+      kk::model_export_slice(m, h, by_ptr);
+    }
   });
 }
 
@@ -199,12 +213,10 @@ int kk_peer_attach_buffer(kk_model* m, int rank, int which, const void* h) {
   return guard([&] {
     need(m, "model");
     need(h, "ipc_handle");
-    if (which == KK_BUF_POOL) kk::model_peer_attach(m, rank, h, true);
-    else if (which == KK_BUF_POOL_PTR) kk::model_peer_attach(m, rank, h, false);
-    else if (which == KK_BUF_RAW) kk::model_peer_attach_raw(m, rank, h);
-    else if (which == KK_BUF_SLICE) kk::model_peer_attach_slice(m, rank, h, true);
-    else if (which == KK_BUF_SLICE_PTR) kk::model_peer_attach_slice(m, rank, h, false);
-    else kk::fail(KK_EINVAL, "unknown buffer kind %d", which);
+    kk::PeerKind kind;
+    bool by_ptr;
+    if (!buf_kind(which, kind, by_ptr)) kk::fail(KK_EINVAL, "unknown buffer kind %d", which);
+    kk::model_peer_attach(m, kind, rank, h, !by_ptr);
   });
 }
 
@@ -502,7 +514,10 @@ int kk_probe_peer(kk_model* m, int rank, int which, uint64_t* nbytes, float* ms)
     need(nbytes, "nbytes");
     need(ms, "ms");
     *ms = 0.f;
-    kk::model_probe_peer(m, rank, which, *nbytes, ms);
+    kk::PeerKind kind;
+    bool by_ptr;
+    if (!buf_kind(which, kind, by_ptr) || by_ptr) kk::fail(KK_EINVAL, "probe: buffer kind %d (KK_BUF_POOL, KK_BUF_RAW or KK_BUF_SLICE)", which);
+    kk::model_probe_peer(m, rank, kind, *nbytes, ms);
   });
 }
 

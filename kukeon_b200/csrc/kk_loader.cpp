@@ -1,24 +1,16 @@
-// Host side of the loader: staging pipeline (pread -> pinned ring -> H2D -> convert/fan-out kernel),
+// Host side of the loader: staging pipeline (page cache -> pinned ring -> H2D -> convert/fan-out kernel),
 // pool allocation, refcounted model registry, IPC export, resident-image measurement mode.
 //
-// Pipeline per ingesting device (SURVEY.md §8(a3.S2-S4)):
+// Pipeline per ingesting device (SURVEY.md §8(a3.S2-S4)), stream_part:
 //   R reader threads, each with its own CUDA stream and >= 2 pinned slots (+ matching device staging
-//   buffers).  A thread claims the next chunk, waits for its slot's previous kernel (event), preads the
-//   chunk's file ranges into the pinned slot, enqueues H2D + the convert kernel on its stream and moves
-//   on.  Disk/page-cache reads, PCIe DMA and the kernels of different threads overlap.  The kernel writes
+//   buffers).  A thread claims the next chunk, waits for its slot's previous work (event), reads the
+//   chunk's file ranges into the pinned slot (kk_read.cpp), enqueues what moves the chunk on (H2D, launches) on its stream and moves
+//   on.  Disk/page-cache reads, PCIe DMA and the kernels of different threads overlap.  In a streaming load the convert kernel writes
 //   bf16 into the local pool and, in BROADCAST mode, into every peer pool over NVLink in the same pass.
 #include "kk_loader.hpp"
 
-#include <fcntl.h>
-#if defined(__x86_64__)
-#include <immintrin.h>
-#endif
 #include <pthread.h>
 #include <sched.h>
-#include <sys/mman.h>
-#include <sys/stat.h>
-#include <sys/vfs.h>
-#include <unistd.h>
 
 #include <algorithm>
 #include <chrono>
@@ -28,6 +20,13 @@
 #include <thread>
 
 #include "kk_json.hpp"
+#include "kk_read.hpp"
+
+// A host test that #includes this file whole, to reach the functions of its anonymous namespace, links the library's other objects but not
+// kk_read.o: such a translation unit compiles the read path in with this file.  The library itself links kk_read.o.
+#if __INCLUDE_LEVEL__ > 0
+#include "kk_read.cpp"
+#endif
 
 namespace kk {
 
@@ -35,72 +34,6 @@ namespace {
 
 double now_s() {
   return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count();
-}
-
-struct FdSet {
-  enum MapPolicy { kMapNone = 0, kMapTmpfs, kMapAll };  // which shards get a read-only mapping next to their descriptor
-  std::vector<int> fds;
-  std::vector<const uint8_t*> maps;  // read-only mappings (nullptr = none): long ranges are copied out of them with streaming stores, see read_chunk
-  std::vector<uint64_t> sizes;
-  explicit FdSet(const std::vector<std::string>& paths, MapPolicy policy = kMapNone) {
-    for (auto& p : paths) {
-      int fd = ::open(p.c_str(), O_RDONLY | O_CLOEXEC);
-      if (fd < 0) {
-        int e = errno;
-        cleanup();
-        fail(e == ENOENT ? KK_ENOENT : KK_EIO, "open %s: %s", p.c_str(), strerror(e));
-      }
-      fds.push_back(fd);
-      const uint8_t* mp = nullptr;
-      uint64_t sz = 0;
-      bool want = policy == kMapAll;
-      if (policy == kMapTmpfs) {
-        struct statfs sf;
-        want = fstatfs(fd, &sf) == 0 && (unsigned long)sf.f_type == 0x01021994ul;  // TMPFS_MAGIC: every byte is in memory, a mapping never waits for a disk
-      }
-      if (want) {
-        struct stat st;
-        if (fstat(fd, &st) == 0 && st.st_size > 0) {
-          void* m = mmap(nullptr, (size_t)st.st_size, PROT_READ, MAP_SHARED, fd, 0);
-          if (m != MAP_FAILED) { mp = (const uint8_t*)m; sz = (uint64_t)st.st_size; }
-        }
-      }
-      maps.push_back(mp);
-      sizes.push_back(sz);
-    }
-  }
-  // Bytes of shard i that may be read through its mapping right now: touching a mapped page past the end of a file that has been truncated since
-  // it was mapped raises SIGBUS, where pread reports a short read.  Asked once per chunk (one fstat per 16 MiB), this narrows that window from the
-  // whole load to one chunk's copy; a range beyond the returned size takes the pread path and its KK_EIO.
-  uint64_t live_size(uint32_t i) const {
-    struct stat st;
-    if (fstat(fds[i], &st) != 0 || st.st_size < 0) return 0;
-    return std::min<uint64_t>((uint64_t)st.st_size, sizes[i]);
-  }
-  void cleanup() {
-    for (size_t i = 0; i < maps.size(); ++i)
-      if (maps[i]) munmap((void*)maps[i], sizes[i]);
-    for (int f : fds) ::close(f);
-    maps.clear();
-    fds.clear();
-  }
-  ~FdSet() { cleanup(); }
-  FdSet(const FdSet&) = delete;
-  FdSet& operator=(const FdSet&) = delete;
-};
-
-void pread_full(int fd, uint8_t* dst, uint64_t len, uint64_t off, const std::string& name) {
-  while (len) {
-    ssize_t r = ::pread(fd, dst, len > (1ull << 30) ? (1ull << 30) : len, (off_t)off);
-    if (r < 0) {
-      if (errno == EINTR) continue;
-      fail(KK_EIO, "pread %s @%llu: %s", name.c_str(), (unsigned long long)off, strerror(errno));
-    }
-    if (r == 0) fail(KK_EIO, "pread %s @%llu: unexpected end of file", name.c_str(), (unsigned long long)off);
-    dst += r;
-    off += (uint64_t)r;
-    len -= (uint64_t)r;
-  }
 }
 
 // CPUs of the NUMA node the device hangs off (empty when sysfs does not say).
@@ -180,88 +113,59 @@ struct DevScratch {
   }
 };
 
-// How a chunk's long contiguous ranges travel from the page cache into the pinned slot (Llama-3-8B from tmpfs, 16 reader threads):
-//   pread                       the kernel's copy_to_user, 4 KiB at a time: the load is reader-bound
-//   mapping + memcpy            no faster than pread, and the final munmap of a checkpoint-sized mapping is ONE thread tearing down 4 M page-table
-//                               entries
-//   mapping + streaming stores  about half pread's copy time per thread (no read-for-ownership of the slot's lines, which only the DMA engine
-//                               reads next) — with the same munmap bill
-//   ... + MADV_DONTNEED of each range right after its copy (the reader threads drop their own page-table entries in parallel, the final munmap
-//                               finds none): the load becomes H2D-bound.  DEFAULT for shards on tmpfs; other file systems keep pread (a mapping of
-//                               a cold file would fault page by page into the disk).
-//   MAP_POPULATE mapping per range: slower than pread (every mmap / munmap takes the process's mm lock exclusively).
-//   cache-resident bounce ring (4 x 256 KiB pinned pieces per reader between mapping and device slot, so that neither the CPU's stores nor the copy
-//                               engine's reads reach DRAM): faster CPU copy, but 64 K small H2D copies starve the copy engines.
-// The slower forms are deleted (git history: ed69c4b..50a97f8 carry them); what is left is the default and one switch:
-// KUKEON_GPULOAD_READ = pread (never map) | mapped (map every shard, whatever the file system).  Measurement knob, not API.
-enum ReadMode { kReadAuto = 0, kReadPread, kReadMapped };
-ReadMode read_mode() {
-  static const ReadMode mode = [] {
-    const char* e = getenv("KUKEON_GPULOAD_READ");
-    if (!e) return kReadAuto;
-    if (!strcmp(e, "pread")) return kReadPread;
-    if (!strcmp(e, "mapped")) return kReadMapped;
-    return kReadAuto;
-  }();
-  return mode;
-}
-FdSet::MapPolicy map_policy(const kk_model* m) {
-  switch (read_mode()) {
-    case kReadAuto: return FdSet::kMapTmpfs;
-    case kReadPread: return FdSet::kMapNone;
-    default: return FdSet::kMapAll;
-  }
-}
-#if defined(__x86_64__)
-__attribute__((target("avx2"))) void copy_nt_avx2(uint8_t* dst, const uint8_t* src, size_t n) {
-  size_t head = (32u - ((uintptr_t)dst & 31u)) & 31u;
-  if (head > n) head = n;
-  if (head) { memcpy(dst, src, head); dst += head; src += head; n -= head; }
-  size_t i = 0;
-  for (; i + 128 <= n; i += 128) {
-    const __m256i a = _mm256_loadu_si256((const __m256i*)(src + i)), b = _mm256_loadu_si256((const __m256i*)(src + i + 32));
-    const __m256i c = _mm256_loadu_si256((const __m256i*)(src + i + 64)), d = _mm256_loadu_si256((const __m256i*)(src + i + 96));
-    _mm256_stream_si256((__m256i*)(dst + i), a);
-    _mm256_stream_si256((__m256i*)(dst + i + 32), b);
-    _mm256_stream_si256((__m256i*)(dst + i + 64), c);
-    _mm256_stream_si256((__m256i*)(dst + i + 96), d);
-  }
-  if (i < n) memcpy(dst + i, src + i, n - i);
-  _mm_sfence();  // the streaming stores must be globally visible before the H2D copy of the slot is enqueued
-}
-#endif
-void copy_nt(uint8_t* dst, const uint8_t* src, size_t n) {
-#if defined(__x86_64__)
-  static const bool avx2 = __builtin_cpu_supports("avx2");
-  if (avx2) { copy_nt_avx2(dst, src, n); return; }
-#endif
-  memcpy(dst, src, n);
-}
-
-// Fill the slot with the chunk's file bytes.
-void read_chunk(const Chunk& c, const FdSet& fds, const Index& ix, uint8_t* pinned) {
-  static const uint64_t pg = (uint64_t)sysconf(_SC_PAGESIZE);
-  const uint8_t* mp = fds.maps.empty() ? nullptr : fds.maps[c.shard];
-  const uint64_t msz = mp ? fds.live_size(c.shard) : 0;
-  const ReadMode mode = read_mode();
-  for (auto& r : c.reads) {
-    const bool in_map = mp && r.file_off <= msz && r.len <= msz - r.file_off;  // (a file that shrank since it was mapped takes pread's error path)
-    if (in_map && r.len > (256u << 10) && mode != kReadPread) {
-      copy_nt(pinned + r.buf_off, mp + r.file_off, r.len);
-      const uint64_t a = (r.file_off + pg - 1) & ~(pg - 1), e = (r.file_off + r.len) & ~(pg - 1);  // the whole pages inside the range
-      if (e > a) madvise((void*)(mp + a), (size_t)(e - a), MADV_DONTNEED);  // page-table entries only: the pages stay in the page cache
-      continue;
-    }
-    // short ranges (column-slice rows of a SCATTER load: thousands of 2-7 KB runs per chunk) stay on pread: copied out of the mapping the 70B
-    // scatter load is slower — a first-touch page fault per row costs more than the syscall
-    pread_full(fds.fds[c.shard], pinned + r.buf_off, r.len, r.file_off, ix.shards[c.shard]);
-  }
+// Device copy of a segment table on the current device (nullptr for an empty table); the caller frees it.
+KKSeg* upload_segs(const std::vector<KKSeg>& segs) {
+  KKSeg* d = nullptr;
+  if (segs.empty()) return d;
+  KK_CUDA(cudaMalloc((void**)&d, segs.size() * sizeof(KKSeg)));
+  const cudaError_t e = cudaMemcpy(d, segs.data(), segs.size() * sizeof(KKSeg), cudaMemcpyHostToDevice);
+  if (e != cudaSuccess) cudaFree(d);
+  KK_CUDA(e);
+  return d;
 }
 
 uint64_t seg_base_of(const Plan& P, int part) {
   uint64_t b = 0;
   for (int i = 0; i < part; ++i) b += P.parts[(size_t)i].segs.size();
   return b;
+}
+
+// The chunk buffers of plan parts laid out back to back in one device image, and their segments rebased onto it.
+struct ImageLayout {
+  std::vector<std::vector<uint64_t>> chunk_off;  // [i][ci]: offset of chunk ci of parts[i] in the image
+  uint64_t bytes = 0;
+  std::vector<KKSeg> segs;                       // src_off rebased onto the image, tile_begin onto the segment's launch
+  std::vector<ImageLaunch> launches;
+};
+
+// Every chunk takes its staging bytes plus 64 bytes of over-read slack, at a 256-byte boundary.  One launch per shard, split only where a
+// launch would exceed kMaxSegsPerLaunch segments or 0xFFFFFFF0 tiles: kk_convert_resident reports one time per launch.
+ImageLayout lay_out_image(const Plan& P, const std::vector<int>& parts) {
+  ImageLayout im;
+  int last_shard = -1;
+  for (int part : parts) {
+    const PartPlan& pp = P.parts[(size_t)part];
+    im.chunk_off.emplace_back();
+    for (const Chunk& ch : pp.chunks) {
+      const uint64_t off = im.bytes;
+      im.chunk_off.back().push_back(off);
+      im.bytes += align_up(ch.buf_bytes + 64, 256);
+      if (im.launches.empty() || last_shard != (int)ch.shard || im.launches.back().n_segs + ch.seg_count > kMaxSegsPerLaunch ||
+          (uint64_t)im.launches.back().n_tiles + ch.n_tiles > 0xFFFFFFF0ull)
+        im.launches.push_back({(uint32_t)im.segs.size(), 0, 0});
+      last_shard = (int)ch.shard;
+      ImageLaunch& L = im.launches.back();
+      for (uint32_t j = 0; j < ch.seg_count; ++j) {
+        KKSeg sg = pp.segs[ch.seg_begin + j];
+        sg.src_off += off;
+        sg.tile_begin += L.n_tiles;
+        im.segs.push_back(sg);
+      }
+      L.n_segs += ch.seg_count;
+      L.n_tiles += ch.n_tiles;
+    }
+  }
+  return im;
 }
 
 // Test hook: KUKEON_GPULOAD_TEST_NDST=<n> pads the destination list to n entries by repeating the ones it has,
@@ -280,18 +184,13 @@ void pad_dsts_for_test(ConvertLaunch& L) {
 bool is_nvls(const kk_model* m) { return m->opts.fanout == KK_FANOUT_NVLS && m->plan.mode == KK_MODE_BROADCAST && m->nvls; }
 
 // multimem.st exists for 4-, 8- and 16-byte accesses only: a plan qualifies for KK_LAUNCH_MULTIMEM when no segment ever needs a 1- or
-// 2-byte store — every tile of it is whole 16-byte output vectors.  (Block dequantisers and the FP8/F16/F32 casts of whole groups
-// always are; verbatim copies need a multiple of 16 bytes; transposes store single elements at tile edges and are excluded.)
+// 2-byte store — every tile of it is whole 16-byte output vectors.  Transposes store single elements at tile edges and are excluded; FP8
+// widening works on 16-element groups and needs whole groups.
 bool plan_allows_multimem(const Plan& P, std::string* why) {
   for (auto& pp : P.parts)
     for (auto& s : pp.segs) {
-      bool ok;
-      switch (s.op) {
-        case KK_OP_COPY: case KK_OP_F8E4M3_BF16: case KK_OP_F8E5M2_BF16: ok = s.units % 16 == 0; break;
-        case KK_OP_F32_BF16: case KK_OP_F16_BF16: ok = s.units % 8 == 0; break;
-        default: ok = kk_block_geom(s.op).block_bytes != 0; break;
-      }
-      if (!ok) {
+      const bool f8 = s.op == KK_OP_F8E4M3_BF16 || s.op == KK_OP_F8E5M2_BF16;
+      if (kk_is_transpose(s.op) || s.op == KK_OP_ROWSPLIT || seg_out_extent(s) % 16 != 0 || (f8 && s.units % 16 != 0)) {
         if (why) *why = "a tensor's size is not a whole number of 16-byte output vectors (or the load transposes); multimem.st cannot store its tail";
         return false;
       }
@@ -300,26 +199,19 @@ bool plan_allows_multimem(const Plan& P, std::string* why) {
 }
 
 bool is_pull(const kk_model* m) { return m->opts.fanout == KK_FANOUT_PULL && m->plan.mode == KK_MODE_BROADCAST; }
+bool is_raw(const kk_model* m) { return m->opts.fanout == KK_FANOUT_RAW && m->plan.mode == KK_MODE_BROADCAST; }
 
 // Pool bytes [lo, hi) that plan part `part` produces.  Pool order equals file order, so for every op that writes its output
 // linearly this is one contiguous range and the ranges of different parts are disjoint.  Returns false when the part carries ops
-// whose output is not linear in the pool (transposes, the scatter row exchange): such plans cannot be pulled slice by slice.
+// whose output is not linear in the pool (the scatter row exchange; transposes, whose strided stores interleave with the other parts'
+// inside the tensor-wide extent stats() reports for them): such plans cannot be pulled slice by slice.
 bool part_pool_range(const Plan& P, int part, uint64_t& lo, uint64_t& hi) {
   lo = UINT64_MAX;
   hi = 0;
   for (auto& s : P.parts[(size_t)part].segs) {
-    uint64_t e;
-    switch (s.op) {
-      case KK_OP_COPY: e = s.dst_off + s.units; break;
-      case KK_OP_F32_BF16: case KK_OP_F16_BF16: case KK_OP_F8E4M3_BF16: case KK_OP_F8E5M2_BF16: e = s.dst_off + s.units * 2; break;
-      default: {
-        const KKBlockGeom g = kk_block_geom(s.op);
-        if (!g.block_bytes) return false;
-        e = s.dst_off + s.units * g.out_bytes;
-      }
-    }
-    if (s.dst_off < lo) lo = s.dst_off;
-    if (e > hi) hi = e;
+    if (kk_is_transpose(s.op) || s.op == KK_OP_ROWSPLIT) return false;
+    lo = std::min(lo, s.dst_off);
+    hi = std::max(hi, s.dst_off + seg_out_extent(s));
   }
   if (lo == UINT64_MAX) lo = hi = 0;
   return true;
@@ -338,7 +230,7 @@ void fill_dsts(kk_model* m, int li, ConvertLaunch& L) {
     const int n = m->plan.n_parts;
     for (int j = 0; j < n; ++j) {
       uint8_t* p = nullptr;
-      if (m->opts.part_count > 1) p = (j == m->opts.part_index) ? m->pools[0] : (uint8_t*)m->peer_ptr[j];
+      if (m->opts.part_count > 1) p = (j == m->opts.part_index) ? m->pools[0] : (uint8_t*)m->peer[kPeerPool][j].ptr;
       else if (m->ctx->peer_ok) p = m->pools[(size_t)j];
       if (!p) fail(KK_ESTATE, "KK_LOAD_SCATTER_EXCHANGE: the pool of rank %d is not reachable (attach it with kk_peer_attach, or enable peer access)", j);
       L.xdst[j] = p;
@@ -360,8 +252,8 @@ void fill_dsts(kk_model* m, int li, ConvertLaunch& L) {
     return;
   }
   if (m->opts.part_count > 1) {
-    for (int r = 0; r < KK_MAX_DEVICES; ++r)
-      if (m->peer_ptr[r]) L.dst[L.n_dst++] = (uint8_t*)m->peer_ptr[r];
+    for (auto& b : m->peer[kPeerPool])
+      if (b.ptr) L.dst[L.n_dst++] = (uint8_t*)b.ptr;
   } else if (m->ctx->peer_ok) {
     for (size_t j = 0; j < m->pools.size(); ++j)
       if ((int)j != li) L.dst[L.n_dst++] = m->pools[j];
@@ -369,32 +261,42 @@ void fill_dsts(kk_model* m, int li, ConvertLaunch& L) {
   pad_dsts_for_test(L);
 }
 
-// Tile scheduling of a launch: dynamic (counters of the launching stream) for every plan.  On H100 this includes the transposing loads: the
-// GPT-2-small load takes 0.51 ms with dynamic draws against 0.70 ms under static round-robin (one H100 SXM, 700 W limit, 50 launches each,
-// twice, same build).
-uint32_t* sched_for(const kk_model* m, uint32_t* stream_counters) {
-  // measurement knob (A/B of the two schedulers on one box; not part of the API): KUKEON_GPULOAD_SCHED=static | dynamic forces one
-  static const int forced = [] {
-    const char* e = getenv("KUKEON_GPULOAD_SCHED");
-    return !e ? 0 : !strcmp(e, "static") ? 1 : !strcmp(e, "dynamic") ? 2 : 0;
-  }();
-  if (forced == 1) return nullptr;
-  if (forced == 2) return stream_counters;
-  (void)m;
-  return stream_counters;
+// Peer raw images a stage-1 copy launch on local device li writes to (never the local image: it is the source).
+void fill_raw_dsts(kk_model* m, int li, ConvertLaunch& L) {
+  L.n_dst = 0;
+  L.flags = 0;
+  for (auto& d : L.dst) d = nullptr;
+  if (m->opts.part_count > 1) {
+    for (auto& b : m->peer[kPeerRaw])
+      if (b.ptr) L.dst[L.n_dst++] = (uint8_t*)b.ptr;
+  } else {
+    for (size_t j = 0; j < m->raw.size(); ++j)
+      if ((int)j != li) L.dst[L.n_dst++] = m->raw[j].image;
+  }
 }
 
-// Ingest plan part `part` on local device `li`.
-void run_part(kk_model* m, int li, int part, const FdSet& fds) {
+// Tile scheduling of a launch: dynamic (counters of the launching stream) for every plan.  On H100 this includes the transposing loads: the
+// GPT-2-small load takes 0.51 ms with dynamic draws against 0.70 ms under static round-robin (one H100 SXM, 700 W limit, 50 launches each,
+// twice, same build).  KUKEON_GPULOAD_SCHED=static forces static round-robin: a measurement knob for A/B runs of the two schedulers on one
+// box, not part of the API.
+uint32_t* sched_for(uint32_t* stream_counters) {
+  static const bool force_static = [] {
+    const char* e = getenv("KUKEON_GPULOAD_SCHED");
+    return e && !strcmp(e, "static");
+  }();
+  return force_static ? nullptr : stream_counters;
+}
+
+// Stream plan part `part` through the reader threads of local device `li`.  Each thread claims the next chunk, waits until its next slot's
+// previous work has run, reads the chunk into the pinned slot and calls consume(reader, slot, chunk index), which enqueues on the reader's
+// stream what moves the bytes on; the slot is free again once that has run.  record_times: this is the streaming pass of kk_load_part, whose
+// reader timings stats() reports.
+template <class Consume>
+void stream_part(kk_model* m, int li, int part, const FdSet& fds, bool record_times, const Consume& consume) {
   kk_ctx* c = m->ctx;
   Device& dev = c->devs[(size_t)m->dev_idx[(size_t)li]];
   const PartPlan& pp = m->plan.parts[(size_t)part];
-  if (pp.chunks.empty()) return;
   std::lock_guard<std::mutex> pipeline(*dev.load_mu);
-  const KKSeg* d_segs = m->d_segs[(size_t)li] + seg_base_of(m->plan, part);
-  ConvertLaunch base{};
-  fill_dsts(m, li, base);
-  const bool zerocopy = (c->cfg.flags & KK_CFG_ZEROCOPY) != 0;
   std::atomic<size_t> next{0};
   ErrorSink sink;
   auto ns = [] { return (uint64_t)std::chrono::duration_cast<std::chrono::nanoseconds>(std::chrono::steady_clock::now().time_since_epoch()).count(); };
@@ -406,40 +308,32 @@ void run_part(kk_model* m, int li, int part, const FdSet& fds) {
       uint64_t w_ns = 0, p_ns = 0, i_ns = 0;
       for (;;) {
         if (sink.stop) break;
-        size_t ci = next.fetch_add(1);
+        const size_t ci = next.fetch_add(1);
         if (ci >= pp.chunks.size()) break;
-        const Chunk& ch = pp.chunks[ci];
         Slot& s = rd->slots[k++ % rd->slots.size()];
         const uint64_t t0 = ns();
         KK_CUDA(cudaEventSynchronize(s.done));
         const uint64_t t1 = ns();
-        read_chunk(ch, fds, m->plan.index, s.pinned);
+        read_chunk(pp.chunks[ci], fds, m->plan.index, s.pinned);
         const uint64_t t2 = ns();
-        ConvertLaunch L = base;
-        if (zerocopy) {
-          L.src = s.pinned;
-        } else {
-          KK_CUDA(cudaMemcpyAsync(s.dev, s.pinned, ch.buf_bytes, cudaMemcpyHostToDevice, rd->stream));
-          L.src = s.dev;
-        }
-        L.segs = d_segs + ch.seg_begin;
-        L.n_segs = ch.seg_count;
-        L.n_tiles = ch.n_tiles;
-        L.sched = sched_for(m, rd->sched);
-        KK_CUDA(launch_convert(L, dev.sm_count, rd->stream));
+        consume(*rd, s, ci);
         KK_CUDA(cudaEventRecord(s.done, rd->stream));
         w_ns += t1 - t0; p_ns += t2 - t1; i_ns += ns() - t2;
       }
       const uint64_t t3 = ns();
       KK_CUDA(cudaStreamSynchronize(rd->stream));
-      m->rd_drain_ns += ns() - t3;
-      m->rd_wait_ns += w_ns; m->rd_pread_ns += p_ns; m->rd_issue_ns += i_ns;
+      if (record_times) {
+        m->rd_drain_ns += ns() - t3;
+        m->rd_wait_ns += w_ns; m->rd_pread_ns += p_ns; m->rd_issue_ns += i_ns;
+      }
     } catch (...) {
       sink.capture();
     }
   };
-  m->rd_wait_ns = 0; m->rd_pread_ns = 0; m->rd_issue_ns = 0; m->rd_drain_ns = 0;
-  m->rd_threads = (uint32_t)dev.readers.size();
+  if (record_times) {
+    m->rd_wait_ns = 0; m->rd_pread_ns = 0; m->rd_issue_ns = 0; m->rd_drain_ns = 0;
+    m->rd_threads = (uint32_t)dev.readers.size();
+  }
   std::vector<std::thread> th;
   // every reader runs on its own (NUMA-pinned) thread; the caller's thread affinity is left alone
   for (size_t r = 0; r < dev.readers.size(); ++r) th.emplace_back(worker, &dev.readers[r]);
@@ -452,120 +346,81 @@ void run_part(kk_model* m, int li, int part, const FdSet& fds) {
   sink.rethrow();
 }
 
-// ---- KK_FANOUT_RAW ------------------------------------------------------------------------------
-bool is_raw(const kk_model* m) { return m->opts.fanout == KK_FANOUT_RAW && m->plan.mode == KK_MODE_BROADCAST; }
-
-// Peer raw images a stage-1 copy launch on local device li writes to (never the local image: it is the source).
-void fill_raw_dsts(kk_model* m, int li, ConvertLaunch& L) {
-  L.n_dst = 0;
-  L.flags = 0;
-  for (auto& d : L.dst) d = nullptr;
-  if (m->opts.part_count > 1) {
-    for (int r = 0; r < KK_MAX_DEVICES; ++r)
-      if (m->peer_raw_ptr[r]) L.dst[L.n_dst++] = (uint8_t*)m->peer_raw_ptr[r];
-  } else {
-    for (size_t j = 0; j < m->raw.size(); ++j)
-      if ((int)j != li) L.dst[L.n_dst++] = m->raw[j].image;
-  }
-}
-
-// Stage 1 of a RAW load on local device li: file bytes of plan part `part` -> local raw image (H2D straight into
-// place) -> peers' raw images (COPY launch per chunk, bulk TMA stores over NVLink).  fan_out=false: H2D only.
-void run_part_raw(kk_model* m, int li, int part, const FdSet& fds, bool fan_out) {
-  kk_ctx* c = m->ctx;
-  Device& dev = c->devs[(size_t)m->dev_idx[(size_t)li]];
+// Streaming load of plan part `part` on local device li: H2D into the slot's device buffer (or zero-copy), then the convert launch.
+void convert_part(kk_model* m, int li, int part, const FdSet& fds) {
   const PartPlan& pp = m->plan.parts[(size_t)part];
   if (pp.chunks.empty()) return;
-  std::lock_guard<std::mutex> pipeline(*dev.load_mu);
+  const int sm_count = m->ctx->devs[(size_t)m->dev_idx[(size_t)li]].sm_count;
+  const bool zerocopy = (m->ctx->cfg.flags & KK_CFG_ZEROCOPY) != 0;
+  const KKSeg* d_segs = m->d_segs[(size_t)li] + seg_base_of(m->plan, part);
+  ConvertLaunch base{};
+  fill_dsts(m, li, base);
+  stream_part(m, li, part, fds, true, [&](Reader& rd, Slot& s, size_t ci) {
+    const Chunk& ch = pp.chunks[ci];
+    ConvertLaunch L = base;
+    L.src = s.pinned;
+    if (!zerocopy) {
+      KK_CUDA(cudaMemcpyAsync(s.dev, s.pinned, ch.buf_bytes, cudaMemcpyHostToDevice, rd.stream));
+      L.src = s.dev;
+    }
+    L.segs = d_segs + ch.seg_begin;
+    L.n_segs = ch.seg_count;
+    L.n_tiles = ch.n_tiles;
+    L.sched = sched_for(rd.sched);
+    KK_CUDA(launch_convert(L, sm_count, rd.stream));
+  });
+}
+
+// Stage 1 of a RAW load on local device li: file bytes of its plan part -> local raw image (H2D straight into place) -> peers' raw images
+// (COPY launch per chunk, bulk TMA stores over NVLink).
+void raw_stage1(kk_model* m, int li, const FdSet& fds) {
+  const int part = m->local_parts[(size_t)li];
+  const PartPlan& pp = m->plan.parts[(size_t)part];
+  if (pp.chunks.empty()) return;
+  const int sm_count = m->ctx->devs[(size_t)m->dev_idx[(size_t)li]].sm_count;
   kk_model::Raw& R = m->raw[(size_t)li];
   ConvertLaunch base{};
   fill_raw_dsts(m, li, base);
-  const bool do_fan = fan_out && base.n_dst > 0;
-  if (do_fan && !c->peer_ok && m->opts.part_count <= 1) fail(KK_EUNSUPPORTED, "KK_FANOUT_RAW needs peer access between the context's devices");
-  std::atomic<size_t> next{0};
-  ErrorSink sink;
-  auto worker = [&](Reader* rd) {
-    try {
-      if (!(c->cfg.flags & KK_CFG_NO_NUMA_PIN)) pin_this_thread(dev.numa_cpus);
-      KK_CUDA(cudaSetDevice(dev.ordinal));
-      size_t k = 0;
-      for (;;) {
-        if (sink.stop) break;
-        size_t ci = next.fetch_add(1);
-        if (ci >= pp.chunks.size()) break;
-        const Chunk& ch = pp.chunks[ci];
-        Slot& s = rd->slots[k++ % rd->slots.size()];
-        KK_CUDA(cudaEventSynchronize(s.done));
-        read_chunk(ch, fds, m->plan.index, s.pinned);
-        KK_CUDA(cudaMemcpyAsync(R.image + m->img_off[(size_t)part][ci], s.pinned, ch.buf_bytes, cudaMemcpyHostToDevice, rd->stream));
-        if (do_fan) {
-          ConvertLaunch L = base;
-          L.src = R.image;
-          L.segs = R.d_copy_segs + m->chunk_base[(size_t)part] + ci;
-          L.n_segs = 1;
-          L.n_tiles = (uint32_t)kk_seg_tiles(KK_OP_COPY, align_up(ch.buf_bytes, 16), 0);
-          L.sched = sched_for(m, rd->sched);
-        KK_CUDA(launch_convert(L, dev.sm_count, rd->stream));
-        }
-        KK_CUDA(cudaEventRecord(s.done, rd->stream));
-      }
-      KK_CUDA(cudaStreamSynchronize(rd->stream));
-    } catch (...) {
-      sink.capture();
-    }
-  };
-  std::vector<std::thread> th;
-  for (size_t r = 0; r < dev.readers.size(); ++r) th.emplace_back(worker, &dev.readers[r]);
-  for (auto& t : th) t.join();
-  if (sink.first) {
-    cudaSetDevice(dev.ordinal);
-    for (auto& r : dev.readers) cudaStreamSynchronize(r.stream);
-  }
-  sink.rethrow();
+  if (base.n_dst > 0 && !m->ctx->peer_ok && m->opts.part_count <= 1) fail(KK_EUNSUPPORTED, "KK_FANOUT_RAW needs peer access between the context's devices");
+  stream_part(m, li, part, fds, true, [&](Reader& rd, Slot& s, size_t ci) {
+    const Chunk& ch = pp.chunks[ci];
+    KK_CUDA(cudaMemcpyAsync(R.image + m->img_off[(size_t)part][ci], s.pinned, ch.buf_bytes, cudaMemcpyHostToDevice, rd.stream));
+    if (base.n_dst == 0) return;
+    ConvertLaunch L = base;
+    L.src = R.image;
+    L.segs = R.d_copy_segs + m->chunk_base[(size_t)part] + ci;
+    L.n_segs = 1;
+    L.n_tiles = (uint32_t)kk_seg_tiles(KK_OP_COPY, align_up(ch.buf_bytes, 16), 0);
+    L.sched = sched_for(rd.sched);
+    KK_CUDA(launch_convert(L, sm_count, rd.stream));
+  });
+}
+
+// Resident staging (untimed): the chunk buffers of plan part `part`, exactly as the streaming path stages them, into `image` at chunk_off.
+void stage_image(kk_model* m, int li, int part, const FdSet& fds, uint8_t* image, const std::vector<uint64_t>& chunk_off) {
+  const PartPlan& pp = m->plan.parts[(size_t)part];
+  stream_part(m, li, part, fds, false, [&](Reader& rd, Slot& s, size_t ci) {
+    KK_CUDA(cudaMemcpyAsync(image + chunk_off[ci], s.pinned, pp.chunks[ci].buf_bytes, cudaMemcpyHostToDevice, rd.stream));
+  });
 }
 
 // Allocate the raw images and build the stage-1 (copy) and stage-2 (convert) segment tables.
 void setup_raw(kk_model* m) {
   const Plan& P = m->plan;
-  m->img_off.assign(P.parts.size(), {});
+  std::vector<int> all;
+  for (int p = 0; p < (int)P.parts.size(); ++p) all.push_back(p);
+  const ImageLayout im = lay_out_image(P, all);
+  m->img_off = im.chunk_off;
   m->chunk_base.assign(P.parts.size(), 0);
-  uint64_t tot = 0;
-  uint32_t nchunks = 0;
+  std::vector<KKSeg> copy_segs;
   for (size_t p = 0; p < P.parts.size(); ++p) {
-    m->chunk_base[p] = nchunks;
-    for (auto& ch : P.parts[p].chunks) {
-      m->img_off[p].push_back(tot);
-      tot += align_up(ch.buf_bytes + 64, 256);
-      nchunks++;
-    }
-  }
-  std::vector<KKSeg> copy_segs, conv_segs;
-  std::vector<kk_model::Resident::Launch> launches;
-  int last_shard = -1;
-  for (size_t p = 0; p < P.parts.size(); ++p) {
-    const PartPlan& pp = P.parts[p];
-    for (size_t ci = 0; ci < pp.chunks.size(); ++ci) {
-      const Chunk& ch = pp.chunks[ci];
+    m->chunk_base[p] = (uint32_t)copy_segs.size();
+    for (size_t ci = 0; ci < P.parts[p].chunks.size(); ++ci) {
       KKSeg cs{};
       cs.src_off = cs.dst_off = m->img_off[p][ci];
-      cs.units = align_up(ch.buf_bytes, 16);
+      cs.units = align_up(P.parts[p].chunks[ci].buf_bytes, 16);
       cs.op = KK_OP_COPY;
       copy_segs.push_back(cs);
-      bool fresh = launches.empty() || last_shard != (int)ch.shard || launches.back().n_segs + ch.seg_count > kMaxSegsPerLaunch ||
-                   (uint64_t)launches.back().n_tiles + ch.n_tiles > 0xFFFFFFF0ull;
-      if (fresh) launches.push_back({(uint32_t)conv_segs.size(), 0, 0, 0, 0});
-      last_shard = (int)ch.shard;
-      auto& L = launches.back();
-      for (uint32_t j = 0; j < ch.seg_count; ++j) {
-        KKSeg sg = pp.segs[ch.seg_begin + j];
-        sg.src_off += m->img_off[p][ci];
-        sg.tile_begin += L.n_tiles;
-        conv_segs.push_back(sg);
-      }
-      L.n_segs += ch.seg_count;
-      L.n_tiles += ch.n_tiles;
-      L.src_bytes += ch.src_bytes;
-      L.out_bytes += ch.out_bytes;
     }
   }
   m->raw.resize(m->dev_idx.size());
@@ -573,18 +428,12 @@ void setup_raw(kk_model* m) {
     Device& d = m->ctx->devs[(size_t)m->dev_idx[li]];
     KK_CUDA(cudaSetDevice(d.ordinal));
     auto& R = m->raw[li];
-    R.bytes = align_up(tot ? tot : 256, 2u << 20);  // 2 MiB multiples: cheap to map over CUDA IPC (see the slice buffer in model_load)
+    R.bytes = align_up(im.bytes ? im.bytes : 256, 2u << 20);  // 2 MiB multiples: cheap to map over CUDA IPC (see the slice buffer in model_load)
     cudaError_t e = cudaMalloc((void**)&R.image, R.bytes);
     if (e != cudaSuccess) { cudaGetLastError(); R.image = nullptr; fail(KK_ENOMEM, "device %d: cudaMalloc(%llu) for the raw image failed", d.ordinal, (unsigned long long)R.bytes); }
-    if (!copy_segs.empty()) {
-      KK_CUDA(cudaMalloc((void**)&R.d_copy_segs, copy_segs.size() * sizeof(KKSeg)));
-      KK_CUDA(cudaMemcpy(R.d_copy_segs, copy_segs.data(), copy_segs.size() * sizeof(KKSeg), cudaMemcpyHostToDevice));
-    }
-    if (!conv_segs.empty()) {
-      KK_CUDA(cudaMalloc((void**)&R.d_conv_segs, conv_segs.size() * sizeof(KKSeg)));
-      KK_CUDA(cudaMemcpy(R.d_conv_segs, conv_segs.data(), conv_segs.size() * sizeof(KKSeg), cudaMemcpyHostToDevice));
-    }
-    R.conv_launches = launches;
+    R.d_copy_segs = upload_segs(copy_segs);
+    R.d_conv_segs = upload_segs(im.segs);
+    R.conv_launches = im.launches;
   }
 }
 
@@ -599,49 +448,74 @@ void free_raw(kk_model* m) {
   m->raw.clear();
 }
 
-// Stage 2: every local device converts the whole gathered image into its own pool.
-void convert_local_all(kk_model* m, float* ms_total) {
-  kk_ctx* c = m->ctx;
-  const size_t nl = m->dev_idx.size();
-  EventSet e0(nl), e1(nl);
-  for (size_t li = 0; li < nl; ++li) {
-    Device& dev = c->devs[(size_t)m->dev_idx[li]];
-    auto& R = m->raw[li];
+// The launches over a device image, each with base's destinations.
+std::vector<ConvertLaunch> image_launches(const ConvertLaunch& base, const uint8_t* image, const KKSeg* d_segs, const std::vector<ImageLaunch>& launches) {
+  std::vector<ConvertLaunch> out;
+  for (auto& la : launches) {
+    ConvertLaunch L = base;
+    L.src = image;
+    L.segs = d_segs + la.seg_begin;
+    L.n_segs = la.n_segs;
+    L.n_tiles = la.n_tiles;
+    out.push_back(L);
+  }
+  return out;
+}
+
+// Run launches[li] on the stream of local device li, enqueued on every device before any device is waited for, so that the devices run
+// concurrently.  Events bracket the launches alone.  Returns the slowest device's total (ms); per_launch[k] = the slowest k-th launch.
+float time_launches(kk_model* m, std::vector<std::vector<ConvertLaunch>>& launches, std::vector<float>* per_launch = nullptr) {
+  std::vector<EventSet> evs;
+  evs.reserve(launches.size());
+  size_t most = 0;
+  for (size_t li = 0; li < launches.size(); ++li) {
+    Device& dev = m->ctx->devs[(size_t)m->dev_idx[li]];
     KK_CUDA(cudaSetDevice(dev.ordinal));
-    KK_CUDA(cudaEventCreate(&e0[li]));
-    KK_CUDA(cudaEventCreate(&e1[li]));
-    KK_CUDA(cudaEventRecord(e0[li], dev.stream));
-    for (auto& La : R.conv_launches) {
-      ConvertLaunch L{};
-      L.src = R.image;
-      L.segs = R.d_conv_segs + La.seg_begin;
-      L.n_segs = La.n_segs;
-      L.n_tiles = La.n_tiles;
-      L.n_dst = 1;
-      L.dst[0] = m->pools[li];
-      L.sched = sched_for(m, dev.sched);
-      KK_CUDA(launch_convert(L, dev.sm_count, dev.stream));
+    evs.emplace_back(launches[li].size() + 1);
+    evs[li].create_all();
+    KK_CUDA(cudaEventRecord(evs[li][0], dev.stream));
+    for (size_t k = 0; k < launches[li].size(); ++k) {
+      launches[li][k].sched = sched_for(dev.sched);
+      KK_CUDA(launch_convert(launches[li][k], dev.sm_count, dev.stream));
+      KK_CUDA(cudaEventRecord(evs[li][k + 1], dev.stream));
     }
-    KK_CUDA(cudaEventRecord(e1[li], dev.stream));
+    most = std::max(most, launches[li].size());
   }
   float worst = 0.f;
-  for (size_t li = 0; li < nl; ++li) {
-    Device& dev = c->devs[(size_t)m->dev_idx[li]];
-    KK_CUDA(cudaSetDevice(dev.ordinal));
-    KK_CUDA(cudaStreamSynchronize(dev.stream));
+  if (per_launch) per_launch->assign(most, 0.f);
+  for (size_t li = 0; li < launches.size(); ++li) {
+    KK_CUDA(cudaSetDevice(m->ctx->devs[(size_t)m->dev_idx[li]].ordinal));
+    KK_CUDA(cudaStreamSynchronize(m->ctx->devs[(size_t)m->dev_idx[li]].stream));
+    const size_t n = launches[li].size();
     float ms = 0.f;
-    KK_CUDA(cudaEventElapsedTime(&ms, e0[li], e1[li]));
-    if (ms > worst) worst = ms;
+    KK_CUDA(cudaEventElapsedTime(&ms, evs[li][0], evs[li][n]));
+    worst = std::max(worst, ms);
+    for (size_t k = 0; per_launch && k < n; ++k) {
+      KK_CUDA(cudaEventElapsedTime(&ms, evs[li][k], evs[li][k + 1]));
+      (*per_launch)[k] = std::max((*per_launch)[k], ms);
+    }
   }
-  if (ms_total) *ms_total = worst;
+  return worst;
+}
+
+// Stage 2: every local device converts the whole gathered image into its own pool.
+void convert_local_all(kk_model* m, float* ms_total) {
+  std::vector<std::vector<ConvertLaunch>> launches(m->dev_idx.size());
+  for (size_t li = 0; li < launches.size(); ++li) {
+    ConvertLaunch base{};
+    base.n_dst = 1;
+    base.dst[0] = m->pools[li];
+    launches[li] = image_launches(base, m->raw[li].image, m->raw[li].d_conv_segs, m->raw[li].conv_launches);
+  }
+  const float ms = time_launches(m, launches);
+  if (ms_total) *ms_total = ms;
 }
 
 // Stage 2 of a KK_FANOUT_PULL load: one COPY launch whose segments read every attached peer's slice buffer over NVLink (bulk loads)
 // and write the local pool.  Segments start with the peer after this rank so that the N ranks do not all read GPU 0 first.
 void pull_slices(kk_model* m, float* ms_total) {
-  kk_ctx* c = m->ctx;
-  Device& dev = c->devs[(size_t)m->dev_idx[0]];
   const int n = m->opts.part_count, me = m->opts.part_index;
+  const PeerBuf* slice = m->peer[kPeerSlice];
   std::vector<int> peers;
   std::lock_guard<std::mutex> peer_lock(m->peer_mu);
   // Every rank owns a slice buffer (never smaller than 256 B) and every peer's must be attached before stage 2, whether or not the
@@ -649,26 +523,22 @@ void pull_slices(kk_model* m, float* ms_total) {
   // only because its part happened to be empty (a checkpoint smaller than one staging chunk) would hide the same mistake at full size.
   for (int k = 1; k < n; ++k) {
     const int r = (me + k) % n;
-    if (!m->peer_slice_ptr[r]) fail(KK_ESTATE, "KK_FANOUT_PULL: the slice buffer of rank %d is not attached (kk_peer_attach_buffer, KK_BUF_SLICE)", r);
+    if (!slice[r].ptr) fail(KK_ESTATE, "KK_FANOUT_PULL: the slice buffer of rank %d is not attached (kk_peer_attach_buffer, KK_BUF_SLICE)", r);
     if (m->part_range[(size_t)r].second > m->part_range[(size_t)r].first) peers.push_back(r);
   }
-  KK_CUDA(cudaSetDevice(dev.ordinal));
-  EventSet ev(2);
-  ev.create_all();
-  if (peers.empty()) {
-    KK_CUDA(cudaEventRecord(ev[0], dev.stream));
-    KK_CUDA(cudaEventRecord(ev[1], dev.stream));
-  } else {
+  std::vector<std::vector<ConvertLaunch>> launches(1);
+  DevScratch table;  // freed after time_launches has waited for the launch that reads it
+  if (!peers.empty()) {
     // one src base for the launch: the numerically lowest peer mapping; every segment's src_off is its distance from it
     uintptr_t base = UINTPTR_MAX;
-    for (int r : peers) base = std::min(base, (uintptr_t)m->peer_slice_ptr[r]);
+    for (int r : peers) base = std::min(base, (uintptr_t)slice[r].ptr);
     base &= ~(uintptr_t)15;
     std::vector<KKSeg> segs;
     uint64_t tiles = 0;
     for (int r : peers) {
       const uint64_t lo = m->part_range[(size_t)r].first, hi = m->part_range[(size_t)r].second;
       KKSeg sg{};
-      sg.src_off = (uint64_t)((uintptr_t)m->peer_slice_ptr[r] - base) + (lo - (lo & ~(uint64_t)255));  // peers allocate from slice_base = lo & ~255
+      sg.src_off = (uint64_t)((uintptr_t)slice[r].ptr - base) + (lo - (lo & ~(uint64_t)255));  // peers allocate from slice_base = lo & ~255
       sg.dst_off = lo;
       sg.units = hi - lo;
       sg.op = KK_OP_COPY;
@@ -677,26 +547,47 @@ void pull_slices(kk_model* m, float* ms_total) {
       segs.push_back(sg);
     }
     if (tiles > 0xFFFFFFF0ull) fail(KK_EUNSUPPORTED, "too many tiles for one pull launch");
-    DevScratch tmp;
-    KK_CUDA(cudaMalloc(&tmp.p, segs.size() * sizeof(KKSeg)));
-    KK_CUDA(cudaMemcpyAsync(tmp.p, segs.data(), segs.size() * sizeof(KKSeg), cudaMemcpyHostToDevice, dev.stream));
+    KK_CUDA(cudaSetDevice(m->ctx->devs[(size_t)m->dev_idx[0]].ordinal));
+    table.p = upload_segs(segs);
     ConvertLaunch L{};
     L.src = (const uint8_t*)base;
-    L.segs = (const KKSeg*)tmp.p;
+    L.segs = (const KKSeg*)table.p;
     L.n_segs = (uint32_t)segs.size();
     L.n_tiles = (uint32_t)tiles;
     L.n_dst = 1;
     L.dst[0] = m->pools[0];
-    KK_CUDA(cudaEventRecord(ev[0], dev.stream));
-    L.sched = sched_for(m, dev.sched);
-      KK_CUDA(launch_convert(L, dev.sm_count, dev.stream));
-    KK_CUDA(cudaEventRecord(ev[1], dev.stream));
-    KK_CUDA(cudaStreamSynchronize(dev.stream));  // tmp outlives the launch
+    launches[0].push_back(L);
   }
-  KK_CUDA(cudaStreamSynchronize(dev.stream));
-  float ms = 0.f;
-  KK_CUDA(cudaEventElapsedTime(&ms, ev[0], ev[1]));
+  const float ms = time_launches(m, launches);
   if (ms_total) *ms_total = ms;
+}
+
+// RAW, kernel-stage measurement: stage 1's fan-out without the file reads — one COPY launch over all of local device li's own chunks, from
+// its raw image into every peer image.  table receives the launch's segment table.
+void raw_fanout_launch(kk_model* m, int li, DevScratch& table, std::vector<ConvertLaunch>& out) {
+  ConvertLaunch L{};
+  fill_raw_dsts(m, li, L);
+  const int part = m->local_parts[(size_t)li];
+  const PartPlan& pp = m->plan.parts[(size_t)part];
+  if (L.n_dst == 0 || pp.chunks.empty()) return;
+  std::vector<KKSeg> segs(pp.chunks.size());
+  uint32_t tiles = 0;
+  for (size_t ci = 0; ci < pp.chunks.size(); ++ci) {
+    KKSeg& sg = segs[ci];
+    sg.src_off = sg.dst_off = m->img_off[(size_t)part][ci];
+    sg.units = align_up(pp.chunks[ci].buf_bytes, 16);
+    sg.op = KK_OP_COPY;
+    sg.tile_begin = tiles;
+    tiles += (uint32_t)kk_seg_tiles(KK_OP_COPY, sg.units, 0);
+  }
+  if (segs.size() > kMaxSegsPerLaunch) fail(KK_EUNSUPPORTED, "too many chunks for one raw fan-out launch");
+  KK_CUDA(cudaSetDevice(m->ctx->devs[(size_t)m->dev_idx[(size_t)li]].ordinal));
+  table.p = upload_segs(segs);
+  L.src = m->raw[(size_t)li].image;
+  L.segs = (const KKSeg*)table.p;
+  L.n_segs = (uint32_t)segs.size();
+  L.n_tiles = tiles;
+  out.push_back(L);
 }
 
 void free_resident(kk_model* m) {
@@ -711,33 +602,28 @@ void free_resident(kk_model* m) {
   m->resident.clear();
 }
 
+// Close the peer buffers this process opened over CUDA IPC and forget every attached one.
+void close_peers(kk_model* m) {
+  for (auto& kind : m->peer)
+    for (PeerBuf& b : kind) {
+      if (b.opened_by_ipc) {
+        cudaSetDevice(m->ctx->devs[(size_t)m->dev_idx[0]].ordinal);
+        cudaIpcCloseMemHandle(b.ptr);
+      }
+      b = PeerBuf{};
+    }
+}
+
 void destroy_model(kk_model* m) {
   kk_ctx* c = m->ctx;
+  close_peers(m);
   free_resident(m);
-  for (int r = 0; r < KK_MAX_DEVICES; ++r)
-    if (m->peer_raw_ptr[r]) {
-      cudaSetDevice(c->devs[(size_t)m->dev_idx[0]].ordinal);
-      cudaIpcCloseMemHandle(m->peer_raw_ptr[r]);
-      m->peer_raw_ptr[r] = nullptr;
-    }
   free_raw(m);
-  for (int r = 0; r < KK_MAX_DEVICES; ++r)
-    if (m->peer_slice_ptr[r]) {
-      cudaSetDevice(c->devs[(size_t)m->dev_idx[0]].ordinal);
-      if (m->peer_slice_is_ipc[r]) cudaIpcCloseMemHandle(m->peer_slice_ptr[r]);
-      m->peer_slice_ptr[r] = nullptr;
-    }
   if (m->slice_buf) {
     cudaSetDevice(c->devs[(size_t)m->dev_idx[0]].ordinal);
     cudaFree(m->slice_buf);
     m->slice_buf = nullptr;
   }
-  for (int r = 0; r < KK_MAX_DEVICES; ++r)
-    if (m->peer_ptr[r]) {
-      cudaSetDevice(c->devs[(size_t)m->dev_idx[0]].ordinal);
-      if (m->peer_is_ipc[r]) cudaIpcCloseMemHandle(m->peer_ptr[r]);
-      m->peer_ptr[r] = nullptr;
-    }
   for (size_t i = 0; i < m->pools.size(); ++i) {
     Device& d = c->devs[(size_t)m->dev_idx[i]];
     cudaSetDevice(d.ordinal);
@@ -896,7 +782,7 @@ void ctx_close(kk_ctx* c) {
 // ---------------------------------------------------------------------------------------------
 static void do_load(kk_model* m) {
   const double t0 = now_s();
-  FdSet fds(m->plan.index.shards, map_policy(m));
+  FdSet fds(m->plan.index.shards, map_policy());
   m->t_files_open = now_s() - t0;
   const size_t nl = m->dev_idx.size();
   m->t_part.assign(nl, 0.0);
@@ -908,11 +794,11 @@ static void do_load(kk_model* m) {
     try {
       const double a = now_s();
       if (is_raw(m)) {
-        run_part_raw(m, li, m->local_parts[(size_t)li], fds, true);
+        raw_stage1(m, li, fds);
       } else if (replicas) {
-        for (int p = 0; p < m->plan.n_parts; ++p) run_part(m, li, p, fds);
+        for (int p = 0; p < m->plan.n_parts; ++p) convert_part(m, li, p, fds);
       } else {
-        run_part(m, li, m->local_parts[(size_t)li], fds);
+        convert_part(m, li, m->local_parts[(size_t)li], fds);
       }
       m->t_part[(size_t)li] = now_s() - a;
     } catch (...) {
@@ -1062,10 +948,7 @@ kk_model* model_load(kk_ctx* c, const std::string& path, const kk_load_opts& opt
         m->pool_bytes[li] = 0;
         fail(KK_ENOMEM, "device %d: cudaMalloc(%llu) for the pool failed: %s", d.ordinal, (unsigned long long)pb, cudaGetErrorString(e));
       }
-      if (!all.empty()) {
-        KK_CUDA(cudaMalloc((void**)&m->d_segs[li], all.size() * sizeof(KKSeg)));
-        KK_CUDA(cudaMemcpy(m->d_segs[li], all.data(), all.size() * sizeof(KKSeg), cudaMemcpyHostToDevice));
-      }
+      m->d_segs[li] = upload_segs(all);
     }
     if (is_raw(m)) setup_raw(m);
     if (is_pull(m)) {
@@ -1136,21 +1019,6 @@ void model_export_raw(kk_model* m, int li, void* handle_out) {
   memcpy(handle_out, &h, sizeof h);
 }
 
-void model_peer_attach_raw(kk_model* m, int rank, const void* handle) {
-  std::lock_guard<std::mutex> op(m->op_mu);  // the destination tables are read by a running load
-  if (!is_raw(m)) fail(KK_ESTATE, "raw peer attach needs a KK_FANOUT_RAW model");
-  if (m->opts.part_count <= 1) fail(KK_ESTATE, "peer attach needs a multi-process (part_count > 1) model");
-  if (rank < 0 || rank >= m->opts.part_count || rank == m->opts.part_index) fail(KK_EINVAL, "bad peer rank %d", rank);
-  if (m->peer_raw_ptr[rank]) fail(KK_ESTATE, "peer rank %d already attached", rank);
-  Device& d = m->ctx->devs[(size_t)m->dev_idx[0]];
-  KK_CUDA(cudaSetDevice(d.ordinal));
-  cudaIpcMemHandle_t h;
-  memcpy(&h, handle, sizeof h);
-  void* p = nullptr;
-  KK_CUDA(cudaIpcOpenMemHandle(&p, h, cudaIpcMemLazyEnablePeerAccess));
-  m->peer_raw_ptr[rank] = p;
-}
-
 void model_export_slice(kk_model* m, void* handle_out, bool as_pointer) {
   if (!is_pull(m) || !m->slice_buf) fail(KK_ESTATE, "this model has no slice buffer (KK_FANOUT_PULL only)");
   if (as_pointer) {
@@ -1164,58 +1032,25 @@ void model_export_slice(kk_model* m, void* handle_out, bool as_pointer) {
   memcpy(handle_out, &h, sizeof h);
 }
 
-void model_peer_attach_slice(kk_model* m, int rank, const void* handle, bool is_ipc) {
-  // Not under op_mu: stage 1 of a PULL load (kk_load_part) writes only this rank's own pool and slice buffer, so the caller may map the
-  // peers' slice buffers on another thread while it runs.  The mapping itself happens outside peer_mu (it is the slow part; several
-  // ranks may be attached concurrently), only the table update is locked.
-  if (!is_pull(m)) fail(KK_ESTATE, "slice attach needs a KK_FANOUT_PULL model");
-  if (rank < 0 || rank >= m->opts.part_count || rank == m->opts.part_index) fail(KK_EINVAL, "bad peer rank %d", rank);
-  {
-    std::lock_guard<std::mutex> g(m->peer_mu);
-    if (m->peer_slice_ptr[rank]) fail(KK_ESTATE, "peer rank %d already attached", rank);
-  }
-  KK_CUDA(cudaSetDevice(m->ctx->devs[(size_t)m->dev_idx[0]].ordinal));
-  void* p = nullptr;
-  if (is_ipc) {
-    cudaIpcMemHandle_t h;
-    memcpy(&h, handle, sizeof h);
-    KK_CUDA(cudaIpcOpenMemHandle(&p, h, cudaIpcMemLazyEnablePeerAccess));
-  } else {
-    memcpy(&p, handle, sizeof p);
-    if (!p) fail(KK_EINVAL, "null device pointer");
-  }
-  std::lock_guard<std::mutex> g(m->peer_mu);
-  if (m->peer_slice_ptr[rank]) {  // lost a race against another attach of the same rank
-    if (is_ipc) cudaIpcCloseMemHandle(p);
-    fail(KK_ESTATE, "peer rank %d already attached", rank);
-  }
-  m->peer_slice_ptr[rank] = p;
-  m->peer_slice_is_ipc[rank] = is_ipc;
-}
-
 // NVLink probe (measurement only): copy-engine read of `nbytes` from the attached buffer of rank `rank` (its pool, or its slice buffer
 // in a PULL load) into a local scratch, one untimed pass first, CUDA events on the device's stream.  Run by every rank at once against
 // its ring neighbour this is the per-GPU ingress rate the fan-out's roofline is quoted against — measured in the run, not assumed.
-void model_probe_peer(kk_model* m, int rank, int which, uint64_t& nbytes, float* ms) {
+void model_probe_peer(kk_model* m, int rank, PeerKind kind, uint64_t& nbytes, float* ms) {
   std::lock_guard<std::mutex> op(m->op_mu);
   if (rank < 0 || rank >= KK_MAX_DEVICES) fail(KK_EINVAL, "bad peer rank %d", rank);
-  const uint8_t* src = nullptr;
   uint64_t avail = 0;
-  if (which == KK_BUF_SLICE) {
-    std::lock_guard<std::mutex> g(m->peer_mu);
-    src = (const uint8_t*)m->peer_slice_ptr[rank];
-    if (src && (size_t)rank < m->part_range.size()) {
-      const auto& pr = m->part_range[(size_t)rank];
-      avail = pr.second > (pr.first & ~(uint64_t)255) ? pr.second - (pr.first & ~(uint64_t)255) : 0;
-    }
-  } else if (which == KK_BUF_POOL) {
-    src = (const uint8_t*)m->peer_ptr[rank];
+  if (kind == kPeerPool) {
     avail = m->pool_bytes.empty() ? 0 : m->pool_bytes[0];
-  } else if (which == KK_BUF_RAW) {
-    src = (const uint8_t*)m->peer_raw_ptr[rank];
+  } else if (kind == kPeerRaw) {
     avail = m->raw.empty() ? 0 : m->raw[0].bytes;
-  } else {
-    fail(KK_EINVAL, "probe: buffer kind %d (KK_BUF_POOL, KK_BUF_RAW or KK_BUF_SLICE)", which);
+  } else if ((size_t)rank < m->part_range.size()) {
+    const auto& pr = m->part_range[(size_t)rank];
+    avail = pr.second > (pr.first & ~(uint64_t)255) ? pr.second - (pr.first & ~(uint64_t)255) : 0;
+  }
+  const uint8_t* src;
+  {
+    std::lock_guard<std::mutex> g(m->peer_mu);
+    src = (const uint8_t*)m->peer[kind][rank].ptr;
   }
   if (!src) fail(KK_ESTATE, "probe: rank %d has no attached buffer of that kind", rank);
   nbytes = std::min(nbytes, avail) & ~(uint64_t)255;
@@ -1246,15 +1081,24 @@ void model_release(kk_model* m) {
   destroy_model(m);
 }
 
-void model_peer_attach(kk_model* m, int rank, const void* handle, bool is_ipc) {
-  std::lock_guard<std::mutex> op(m->op_mu);  // the destination tables are read by a running load
+void model_peer_attach(kk_model* m, PeerKind kind, int rank, const void* handle, bool is_ipc) {
+  // Pool and raw tables are read by a running load: those attach under op_mu.  Slice buffers do not: stage 1 of a PULL load (kk_load_part)
+  // writes only this rank's own pool and slice buffer, so the caller may map the peers' slice buffers on another thread while it runs.
+  // The mapping itself happens outside peer_mu (it is the slow part; several ranks may be attached concurrently), only the table update is locked.
+  std::unique_lock<std::mutex> op(m->op_mu, std::defer_lock);
+  if (kind != kPeerSlice) op.lock();
+  if (kind == kPeerRaw && !is_raw(m)) fail(KK_ESTATE, "raw peer attach needs a KK_FANOUT_RAW model");
+  if (kind == kPeerSlice && !is_pull(m)) fail(KK_ESTATE, "slice attach needs a KK_FANOUT_PULL model");
   if (m->opts.part_count <= 1) fail(KK_ESTATE, "peer attach needs a multi-process (part_count > 1) model");
   if (rank < 0 || rank >= m->opts.part_count || rank == m->opts.part_index) fail(KK_EINVAL, "bad peer rank %d", rank);
-  if (m->plan.mode != KK_MODE_BROADCAST && !(m->plan.mode == KK_MODE_SCATTER && (m->plan.flags & KK_LOAD_SCATTER_EXCHANGE)))
+  if (kind == kPeerPool && m->plan.mode != KK_MODE_BROADCAST && !(m->plan.mode == KK_MODE_SCATTER && (m->plan.flags & KK_LOAD_SCATTER_EXCHANGE)))
     fail(KK_ESTATE, "peer attach only applies to BROADCAST models and to SCATTER models loaded with KK_LOAD_SCATTER_EXCHANGE");
-  if (m->peer_ptr[rank]) fail(KK_ESTATE, "peer rank %d already attached", rank);
-  Device& d = m->ctx->devs[(size_t)m->dev_idx[0]];
-  KK_CUDA(cudaSetDevice(d.ordinal));
+  PeerBuf& b = m->peer[kind][rank];
+  {
+    std::lock_guard<std::mutex> g(m->peer_mu);
+    if (b.ptr) fail(KK_ESTATE, "peer rank %d already attached", rank);
+  }
+  KK_CUDA(cudaSetDevice(m->ctx->devs[(size_t)m->dev_idx[0]].ordinal));
   void* p = nullptr;
   if (is_ipc) {
     cudaIpcMemHandle_t h;
@@ -1264,29 +1108,19 @@ void model_peer_attach(kk_model* m, int rank, const void* handle, bool is_ipc) {
     memcpy(&p, handle, sizeof p);
     if (!p) fail(KK_EINVAL, "null device pointer");
   }
-  m->peer_ptr[rank] = p;
-  m->peer_is_ipc[rank] = is_ipc;
+  std::lock_guard<std::mutex> g(m->peer_mu);
+  if (b.ptr) {  // lost a race against a concurrent slice attach of the same rank
+    if (is_ipc) cudaIpcCloseMemHandle(p);
+    fail(KK_ESTATE, "peer rank %d already attached", rank);
+  }
+  b.ptr = p;
+  b.opened_by_ipc = is_ipc;
 }
 
 void model_peer_detach_all(kk_model* m) {
   std::lock_guard<std::mutex> op(m->op_mu);  // the destination tables are read by a running load
   std::lock_guard<std::mutex> pg(m->peer_mu);
-  Device& d = m->ctx->devs[(size_t)m->dev_idx[0]];
-  cudaSetDevice(d.ordinal);
-  for (int r = 0; r < KK_MAX_DEVICES; ++r) {
-    if (m->peer_ptr[r]) {
-      if (m->peer_is_ipc[r]) cudaIpcCloseMemHandle(m->peer_ptr[r]);
-      m->peer_ptr[r] = nullptr;
-    }
-    if (m->peer_raw_ptr[r]) {
-      cudaIpcCloseMemHandle(m->peer_raw_ptr[r]);
-      m->peer_raw_ptr[r] = nullptr;
-    }
-    if (m->peer_slice_ptr[r]) {
-      if (m->peer_slice_is_ipc[r]) cudaIpcCloseMemHandle(m->peer_slice_ptr[r]);
-      m->peer_slice_ptr[r] = nullptr;
-    }
-  }
+  close_peers(m);
 }
 
 int model_local_device(kk_model* m, int ordinal) {
@@ -1375,17 +1209,9 @@ std::string model_stats(kk_model* m) {
     // pool range this part produces (contiguous for SINGLE/BROADCAST because pool order == file order)
     uint64_t lo = UINT64_MAX, hi = 0;
     for (auto& s : pp.segs) {
-      uint64_t b = s.dst_off, e;
-      switch (s.op) {
-        case KK_OP_ROWSPLIT: continue;  // lands in every pool; not part of this rank's contiguous range
-        case KK_OP_COPY: e = b + s.units; break;
-        case KK_OP_F32_BF16: case KK_OP_F16_BF16: case KK_OP_F8E4M3_BF16: case KK_OP_F8E5M2_BF16: e = b + s.units * 2; break;
-        case KK_OP_T_B32: e = b + (uint64_t)s.p0 * s.p1 * 4; break;
-        case KK_OP_T_F32_BF16: case KK_OP_T_F16_BF16: case KK_OP_T_B16: e = b + (uint64_t)s.p0 * s.p1 * 2; break;
-        default: e = b + s.units * kk_block_geom(s.op).out_bytes; break;  // block-dequantising ops
-      }
-      if (b < lo) lo = b;
-      if (e > hi) hi = e;
+      if (s.op == KK_OP_ROWSPLIT) continue;  // lands in every pool; not part of this rank's contiguous range
+      lo = std::min(lo, s.dst_off);
+      hi = std::max(hi, s.dst_off + seg_out_extent(s));
     }
     if (lo == UINT64_MAX) lo = 0;
     uint64_t tiles = 0;
@@ -1404,66 +1230,25 @@ std::string model_stats(kk_model* m) {
 // ---------------------------------------------------------------------------------------------
 void model_stage_resident(kk_model* m) {
   std::lock_guard<std::mutex> op(m->op_mu);
+  if (!is_raw(m)) free_resident(m);
+  else if (m->raw.empty()) fail(KK_ESTATE, "the raw image of this model has been released");
+  FdSet fds(m->plan.index.shards, map_policy());
   if (is_raw(m)) {  // RAW: the resident image IS the raw image; stage this process's own part(s), no fan-out
-    if (m->raw.empty()) fail(KK_ESTATE, "the raw image of this model has been released");
-    FdSet fds(m->plan.index.shards);
-    for (size_t li = 0; li < m->dev_idx.size(); ++li) run_part_raw(m, (int)li, m->local_parts[li], fds, false);
+    for (size_t li = 0; li < m->dev_idx.size(); ++li) stage_image(m, (int)li, m->local_parts[li], fds, m->raw[li].image, m->img_off[(size_t)m->local_parts[li]]);
     return;
   }
-  free_resident(m);
-  kk_ctx* c = m->ctx;
-  FdSet fds(m->plan.index.shards, map_policy(m));
   m->resident.resize(m->dev_idx.size());
   for (size_t li = 0; li < m->dev_idx.size(); ++li) {
-    Device& dev = c->devs[(size_t)m->dev_idx[li]];
+    Device& dev = m->ctx->devs[(size_t)m->dev_idx[li]];
     KK_CUDA(cudaSetDevice(dev.ordinal));
-    const PartPlan& pp = m->plan.parts[(size_t)m->local_parts[li]];
+    const ImageLayout im = lay_out_image(m->plan, {m->local_parts[li]});
     auto& R = m->resident[li];
-    std::vector<uint64_t> img_off(pp.chunks.size());
-    uint64_t tot = 0;
-    for (size_t i = 0; i < pp.chunks.size(); ++i) {
-      img_off[i] = tot;
-      tot += align_up(pp.chunks[i].buf_bytes + 64, 256);
-    }
-    R.image_bytes = tot ? tot : 256;
-    cudaError_t e = cudaMalloc((void**)&R.image, R.image_bytes);
-    if (e != cudaSuccess) { cudaGetLastError(); R.image = nullptr; fail(KK_ENOMEM, "device %d: cudaMalloc(%llu) for the resident image failed", dev.ordinal, (unsigned long long)R.image_bytes); }
-    // copy the chunk bytes exactly as the streaming path stages them
-    std::lock_guard<std::mutex> pipeline(*dev.load_mu);
-    Reader& rd = dev.readers[0];
-    size_t k = 0;
-    for (size_t i = 0; i < pp.chunks.size(); ++i) {
-      Slot& s = rd.slots[k++ % rd.slots.size()];
-      KK_CUDA(cudaEventSynchronize(s.done));
-      read_chunk(pp.chunks[i], fds, m->plan.index, s.pinned);
-      KK_CUDA(cudaMemcpyAsync(R.image + img_off[i], s.pinned, pp.chunks[i].buf_bytes, cudaMemcpyHostToDevice, rd.stream));
-      KK_CUDA(cudaEventRecord(s.done, rd.stream));
-    }
-    KK_CUDA(cudaStreamSynchronize(rd.stream));
-    // one launch per shard (split only if a launch would exceed the segment-table limit)
-    std::vector<KKSeg> segs;
-    for (size_t i = 0; i < pp.chunks.size(); ++i) {
-      const Chunk& ch = pp.chunks[i];
-      bool fresh = R.launches.empty() || pp.chunks[i - 1].shard != ch.shard ||
-                   R.launches.back().n_segs + ch.seg_count > kMaxSegsPerLaunch ||
-                   (uint64_t)R.launches.back().n_tiles + ch.n_tiles > 0xFFFFFFF0ull;
-      if (fresh) R.launches.push_back({(uint32_t)segs.size(), 0, 0, 0, 0});
-      auto& L = R.launches.back();
-      for (uint32_t j = 0; j < ch.seg_count; ++j) {
-        KKSeg s = pp.segs[ch.seg_begin + j];
-        s.src_off += img_off[i];
-        s.tile_begin += L.n_tiles;
-        segs.push_back(s);
-      }
-      L.n_segs += ch.seg_count;
-      L.n_tiles += ch.n_tiles;
-      L.src_bytes += ch.src_bytes;
-      L.out_bytes += ch.out_bytes;
-    }
-    if (!segs.empty()) {
-      KK_CUDA(cudaMalloc((void**)&R.d_segs, segs.size() * sizeof(KKSeg)));
-      KK_CUDA(cudaMemcpy(R.d_segs, segs.data(), segs.size() * sizeof(KKSeg), cudaMemcpyHostToDevice));
-    }
+    const uint64_t bytes = im.bytes ? im.bytes : 256;
+    cudaError_t e = cudaMalloc((void**)&R.image, bytes);
+    if (e != cudaSuccess) { cudaGetLastError(); R.image = nullptr; fail(KK_ENOMEM, "device %d: cudaMalloc(%llu) for the resident image failed", dev.ordinal, (unsigned long long)bytes); }
+    stage_image(m, (int)li, m->local_parts[li], fds, R.image, im.chunk_off[0]);
+    R.d_segs = upload_segs(im.segs);
+    R.launches = im.launches;
   }
 }
 
@@ -1473,123 +1258,30 @@ void model_unstage_resident(kk_model* m) {
   free_resident(m);
 }
 
-// RAW: time the stage-1 fan-out only (own part of the image -> every peer image), one launch per local device.
-static void raw_fanout_resident(kk_model* m, float* ms_total, float* ms_per_launch, size_t cap, size_t* n_launches) {
-  kk_ctx* c = m->ctx;
-  const size_t nl = m->dev_idx.size();
-  EventSet e0(nl), e1(nl);
-  size_t launched = 0;
-  for (size_t li = 0; li < nl; ++li) {
-    Device& dev = c->devs[(size_t)m->dev_idx[li]];
-    KK_CUDA(cudaSetDevice(dev.ordinal));
-    KK_CUDA(cudaEventCreate(&e0[li]));
-    KK_CUDA(cudaEventCreate(&e1[li]));
-    ConvertLaunch L{};
-    fill_raw_dsts(m, (int)li, L);
-    const int part = m->local_parts[li];
-    const PartPlan& pp = m->plan.parts[(size_t)part];
-    KK_CUDA(cudaEventRecord(e0[li], dev.stream));
-    if (L.n_dst > 0 && !pp.chunks.empty()) {
-      // one launch over all of this part's chunks (their COPY segments are consecutive in d_copy_segs)
-      std::vector<KKSeg> segs(pp.chunks.size());
-      uint32_t tiles = 0;
-      for (size_t ci = 0; ci < pp.chunks.size(); ++ci) {
-        KKSeg sg{};
-        sg.src_off = sg.dst_off = m->img_off[(size_t)part][ci];
-        sg.units = align_up(pp.chunks[ci].buf_bytes, 16);
-        sg.op = KK_OP_COPY;
-        sg.tile_begin = tiles;
-        tiles += (uint32_t)kk_seg_tiles(KK_OP_COPY, sg.units, 0);
-        segs[ci] = sg;
-      }
-      if (segs.size() > kMaxSegsPerLaunch) fail(KK_EUNSUPPORTED, "too many chunks for one raw fan-out launch");
-      DevScratch tmp;
-      KK_CUDA(cudaMalloc(&tmp.p, segs.size() * sizeof(KKSeg)));
-      KKSeg* d_tmp = (KKSeg*)tmp.p;
-      KK_CUDA(cudaMemcpyAsync(d_tmp, segs.data(), segs.size() * sizeof(KKSeg), cudaMemcpyHostToDevice, dev.stream));
-      KK_CUDA(cudaEventRecord(e0[li], dev.stream));
-      L.src = m->raw[li].image;
-      L.segs = d_tmp;
-      L.n_segs = (uint32_t)segs.size();
-      L.n_tiles = tiles;
-      L.sched = sched_for(m, dev.sched);
-      KK_CUDA(launch_convert(L, dev.sm_count, dev.stream));
-      KK_CUDA(cudaEventRecord(e1[li], dev.stream));
-      KK_CUDA(cudaStreamSynchronize(dev.stream));  // tmp is freed on scope exit, after the launch that reads it has finished
-      launched = 1;
-    } else {
-      KK_CUDA(cudaEventRecord(e1[li], dev.stream));
-    }
-  }
-  float worst = 0.f;
-  for (size_t li = 0; li < nl; ++li) {
-    Device& dev = c->devs[(size_t)m->dev_idx[li]];
-    KK_CUDA(cudaSetDevice(dev.ordinal));
-    KK_CUDA(cudaStreamSynchronize(dev.stream));
-    float ms = 0.f;
-    KK_CUDA(cudaEventElapsedTime(&ms, e0[li], e1[li]));
-    if (ms > worst) worst = ms;
-  }
-  if (ms_total) *ms_total = worst;
-  if (n_launches) *n_launches = launched;
-  if (ms_per_launch && cap && launched) ms_per_launch[0] = worst;
-}
-
+// RAW: the stage-1 fan-out alone (own part of the image -> every peer image), one launch per local device.  Otherwise the resident image's
+// launches on every local device.
 void model_convert_resident(kk_model* m, float* ms_total, float* ms_per_launch, size_t cap, size_t* n_launches) {
   std::lock_guard<std::mutex> op(m->op_mu);
+  const size_t nl = m->dev_idx.size();
+  std::vector<std::vector<ConvertLaunch>> launches(nl);
+  std::vector<DevScratch> tables(nl);  // RAW: the fan-out launches' segment tables
   if (is_raw(m)) {
     if (m->raw.empty()) fail(KK_ESTATE, "the raw image of this model has been released");
-    raw_fanout_resident(m, ms_total, ms_per_launch, cap, n_launches);
-    return;
-  }
-  if (m->resident.size() != m->dev_idx.size()) fail(KK_ESTATE, "kk_stage_resident has not been called");
-  kk_ctx* c = m->ctx;
-  const size_t nl = m->dev_idx.size();
-  std::vector<EventSet> evs;
-  evs.reserve(nl);
-  size_t max_launches = 0;
-  // enqueue on every local device first (they run concurrently), then collect
-  for (size_t li = 0; li < nl; ++li) {
-    Device& dev = c->devs[(size_t)m->dev_idx[li]];
-    auto& R = m->resident[li];
-    KK_CUDA(cudaSetDevice(dev.ordinal));
-    evs.emplace_back(R.launches.size() + 1);
-    evs[li].create_all();
-    ConvertLaunch base{};
-    fill_dsts(m, (int)li, base);
-    for (size_t k = 0; k < R.launches.size(); ++k) {
-      KK_CUDA(cudaEventRecord(evs[li][k], dev.stream));
-      ConvertLaunch L = base;
-      L.src = R.image;
-      L.segs = R.d_segs + R.launches[k].seg_begin;
-      L.n_segs = R.launches[k].n_segs;
-      L.n_tiles = R.launches[k].n_tiles;
-      L.sched = sched_for(m, dev.sched);
-      KK_CUDA(launch_convert(L, dev.sm_count, dev.stream));
-    }
-    KK_CUDA(cudaEventRecord(evs[li][R.launches.size()], dev.stream));
-    if (R.launches.size() > max_launches) max_launches = R.launches.size();
-  }
-  float worst = 0.f;
-  std::vector<float> per(max_launches, 0.f);
-  for (size_t li = 0; li < nl; ++li) {
-    Device& dev = c->devs[(size_t)m->dev_idx[li]];
-    KK_CUDA(cudaSetDevice(dev.ordinal));
-    KK_CUDA(cudaStreamSynchronize(dev.stream));
-    const size_t n = evs[li].size() - 1;
-    float tot = 0.f;
-    if (n) KK_CUDA(cudaEventElapsedTime(&tot, evs[li][0], evs[li][n]));
-    if (tot > worst) worst = tot;
-    for (size_t k = 0; k < n; ++k) {
-      float ms = 0.f;
-      KK_CUDA(cudaEventElapsedTime(&ms, evs[li][k], evs[li][k + 1]));
-      if (ms > per[k]) per[k] = ms;
+    for (size_t li = 0; li < nl; ++li) raw_fanout_launch(m, (int)li, tables[li], launches[li]);
+  } else {
+    if (m->resident.size() != nl) fail(KK_ESTATE, "kk_stage_resident has not been called");
+    for (size_t li = 0; li < nl; ++li) {
+      ConvertLaunch base{};
+      fill_dsts(m, (int)li, base);
+      launches[li] = image_launches(base, m->resident[li].image, m->resident[li].d_segs, m->resident[li].launches);
     }
   }
-  if (ms_total) *ms_total = worst;
-  if (n_launches) *n_launches = max_launches;
+  std::vector<float> per;
+  const float ms = time_launches(m, launches, &per);
+  if (ms_total) *ms_total = ms;
+  if (n_launches) *n_launches = per.size();
   if (ms_per_launch)
-    for (size_t k = 0; k < max_launches && k < cap; ++k) ms_per_launch[k] = per[k];
+    for (size_t k = 0; k < per.size() && k < cap; ++k) ms_per_launch[k] = per[k];
 }
 
 }  // namespace kk

@@ -51,7 +51,18 @@ struct Device {
   std::vector<int> numa_cpus;  // CPUs local to the device's PCIe root (reader threads are pinned there)
 };
 
-struct Model;
+// Peer buffers of a multi-process model, attached by rank: the other ranks' pools (fan-out destinations), raw images (KK_FANOUT_RAW
+// stage 1) and slice buffers (KK_FANOUT_PULL stage 2).
+enum PeerKind { kPeerPool = 0, kPeerRaw, kPeerSlice, kPeerKinds };
+struct PeerBuf {
+  void* ptr = nullptr;
+  bool opened_by_ipc = false;  // false: a caller-owned device pointer (KK_BUF_*_PTR), never closed by us
+};
+
+// One convert launch over a device image: its slice of the image's rebased segment table.
+struct ImageLaunch {
+  uint32_t seg_begin, n_segs, n_tiles;
+};
 
 }  // namespace kk
 
@@ -82,16 +93,12 @@ struct kk_model {
   std::vector<std::string> manifest_cache;               // per local device, empty = not built yet
   std::vector<std::vector<uint8_t>> pool_handle_cache;   // per local device, empty = not asked yet
   std::vector<KKSeg*> d_segs;        // per local device: device copy of its part's segment table
-  // multi-process fan-out destinations (BROADCAST): IPC-opened peer pools by rank
-  void* peer_ptr[KK_MAX_DEVICES] = {};
-  bool peer_is_ipc[KK_MAX_DEVICES] = {};  // false: caller-owned pointer (KK_BUF_POOL_PTR), never closed by us
+  kk::PeerBuf peer[kk::kPeerKinds][KK_MAX_DEVICES];  // [kind][rank]
   // resident image (kernel-stage measurement)
   struct Resident {
     uint8_t* image = nullptr;
-    uint64_t image_bytes = 0;
     KKSeg* d_segs = nullptr;
-    struct Launch { uint32_t seg_begin, n_segs, n_tiles; uint64_t src_bytes, out_bytes; };
-    std::vector<Launch> launches;
+    std::vector<kk::ImageLaunch> launches;
   };
   std::vector<Resident> resident;  // per local device
   // KK_FANOUT_RAW: the file bytes of every part are all-gathered into a per-device raw image (stage 1, fan-out of
@@ -101,19 +108,16 @@ struct kk_model {
     uint64_t bytes = 0;
     KKSeg* d_copy_segs = nullptr;  // one COPY segment per chunk of every part: [chunk_base[part] + ci]
     KKSeg* d_conv_segs = nullptr;  // every part's segments rebased onto the image
-    std::vector<Resident::Launch> conv_launches;
+    std::vector<kk::ImageLaunch> conv_launches;
   };
   std::vector<Raw> raw;                         // per local device (empty unless fanout == RAW)
   std::vector<std::vector<uint64_t>> img_off;   // [part][chunk] offset of the chunk buffer inside the raw image
   std::vector<uint32_t> chunk_base;             // prefix sum of chunk counts per part
-  void* peer_raw_ptr[KK_MAX_DEVICES] = {};      // IPC-opened raw images of the other ranks
   // KK_FANOUT_PULL (one process per GPU): this rank's part of the pool, [slice_lo, slice_hi), also lives in slice_buf (a separate,
   // small allocation — the only thing peers have to map); slice_buf[0] corresponds to pool offset slice_base
   uint8_t* slice_buf = nullptr;
   uint64_t slice_base = 0;
   std::vector<std::pair<uint64_t, uint64_t>> part_range;  // [lo, hi) pool bytes every part produces
-  void* peer_slice_ptr[KK_MAX_DEVICES] = {};
-  bool peer_slice_is_ipc[KK_MAX_DEVICES] = {};
   bool raw_staged = false;                      // stage 1 complete on this process since the last conversion
   // KK_FANOUT_NVLS (one process, >= 2 devices): the pools are VMM allocations bound to one multicast object; pools[i] then
   // aliases nvls->pool(i) and must not be cudaFree'd
@@ -122,7 +126,7 @@ struct kk_model {
   std::vector<std::unique_ptr<kk::VmmAlloc>> vmm;
   // state
   std::mutex op_mu;  // serialises the data-moving calls on ONE model (kk_load_part, kk_convert_local, kk_*_resident) against each other
-  std::mutex peer_mu;  // guards peer_slice_ptr[]: stage 1 of a PULL load never reads it, so slice buffers may be attached WHILE kk_load_part runs
+  std::mutex peer_mu;  // guards peer[]; slice attach takes only this lock: stage 1 of a PULL load never reads the slice table, so slice buffers may be attached WHILE kk_load_part runs
                        // (cudaIpcOpenMemHandle is the expensive part of time-to-ready in the one-process-per-GPU shape); lock order op_mu -> peer_mu
   int refcount = 0;
   bool loading = true;
@@ -148,13 +152,11 @@ void ctx_close(kk_ctx* c);
 kk_model* model_load(kk_ctx* c, const std::string& path, const kk_load_opts& opts);
 void model_load_part(kk_model* m);
 void model_release(kk_model* m);
-void model_peer_attach(kk_model* m, int rank, const void* handle, bool is_ipc = true);
-void model_peer_attach_raw(kk_model* m, int rank, const void* handle);
+void model_peer_attach(kk_model* m, PeerKind kind, int rank, const void* handle, bool is_ipc);
 void model_export_raw(kk_model* m, int local, void* handle_out);
 void model_export_slice(kk_model* m, void* handle_out, bool as_pointer);
-void model_peer_attach_slice(kk_model* m, int rank, const void* handle, bool is_ipc);
 void model_convert_local(kk_model* m, float* ms_total);
-void model_probe_peer(kk_model* m, int rank, int which, uint64_t& nbytes, float* ms);
+void model_probe_peer(kk_model* m, int rank, PeerKind kind, uint64_t& nbytes, float* ms);
 void model_peer_detach_all(kk_model* m);
 int model_local_device(kk_model* m, int ordinal);  // index into m->dev_idx or throws
 std::string model_manifest(kk_model* m, int local);

@@ -246,6 +246,17 @@ bool is_gpt2_conv1d(const TensorRec& t) {
          ends_with(t.name, "mlp.c_fc.weight") || ends_with(t.name, "mlp.c_proj.weight");
 }
 
+uint64_t seg_out_extent(const KKSeg& s) {
+  switch (s.op) {
+    case KK_OP_ROWSPLIT: return 0;
+    case KK_OP_COPY: return s.units;
+    case KK_OP_F32_BF16: case KK_OP_F16_BF16: case KK_OP_F8E4M3_BF16: case KK_OP_F8E5M2_BF16: return s.units * 2;
+    case KK_OP_T_B32: return (uint64_t)s.p0 * s.p1 * 4;
+    case KK_OP_T_F32_BF16: case KK_OP_T_F16_BF16: case KK_OP_T_B16: return (uint64_t)s.p0 * s.p1 * 2;
+    default: return s.units * kk_block_geom(s.op).out_bytes;  // block-dequantising ops
+  }
+}
+
 uint32_t scatter_slice_dim(const TensorRec& t, int n_parts) {
   if (n_parts <= 1 || t.shape.size() != 2) return kNoSlice;
   const std::string& n = t.name;

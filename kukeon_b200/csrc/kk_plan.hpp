@@ -73,4 +73,9 @@ std::string plan_to_json(const Plan& P);
 // True when KK_LOAD_GPT2_CONV1D_T applies to this tensor.
 bool is_gpt2_conv1d(const TensorRec& t);
 
+// Pool bytes from s.dst_off on that segment s spans in each destination pool.  Copies, casts and block dequantisers fill that range; a
+// transpose spans its whole output tensor but stores only its own rows' columns of it, strided; KK_OP_ROWSPLIT spans nothing here (its
+// rows land in every rank's pool).
+uint64_t seg_out_extent(const KKSeg& s);
+
 }  // namespace kk

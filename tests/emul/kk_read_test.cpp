@@ -1,12 +1,14 @@
-// Host test of the loader's page-cache -> staging-slot read paths (kk_loader.cpp: FdSet, read_chunk, copy_nt) — test infrastructure only.
-// The functions live in kk_loader.cpp's anonymous namespace, so this translation unit includes the source and links against the library's
-// other objects; no CUDA call is made (no GPU needed).  Usage:
+// Host test of the loader's page-cache -> staging-slot read paths (kk_read.cpp: FdSet, read_chunk, copy_nt) — test infrastructure only.
+// Linked against kk_read.o alone; no CUDA (no GPU needed).  Usage:
 //   KUKEON_GPULOAD_READ=<mode> kk_read_test <dir> <policy: none|tmpfs|all> [seed of the random chunks]
 // Writes a pseudo-random file into <dir>, fills a poisoned buffer through read_chunk with a mix of long (> 256 KiB, unaligned) and short ranges,
 // compares every range with the file and every byte outside the ranges with the poison, and prints one JSON line.
-#include "../../kukeon_b200/csrc/kk_loader.cpp"
+#include "kk_read.hpp"
+
+#include <unistd.h>
 
 #include <cstdio>
+#include <cstring>
 #include <random>
 
 using namespace kk;

@@ -379,7 +379,7 @@ def test_medium_checkpoint_checksum_of_checksums(native, tmp_path, coracle):
 
 @pytest.mark.skipif(not os.path.isdir("/dev/shm"), reason="the mapped read path is the default for shards on tmpfs only")
 def test_tmpfs_shards_take_the_mapped_streaming_read_path_bit_exact(pool, coracle):
-    """Shards on tmpfs are read through a mapping with streaming stores and per-range MADV_DONTNEED (kk_loader.cpp read_chunk), everything else with
+    """Shards on tmpfs are read through a mapping with streaming stores and per-range MADV_DONTNEED (kk_read.cpp read_chunk), everything else with
     pread: both must produce the same pool.  An unpadded header puts every range off page and 32-byte boundaries; tensors of 3 B .. 9 MB mix the
     long (> 256 KiB, mapped) and short (pread) ranges in one chunk."""
     d = f"/dev/shm/kk_mapped_{os.getpid()}"
