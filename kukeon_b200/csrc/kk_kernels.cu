@@ -243,10 +243,6 @@ __device__ __forceinline__ KKSeg load_seg(const KKSeg* p) {
   return s;
 }
 
-// DYN: tiles after the first are drawn from L.sched (see the producer); !DYN: static round-robin, the consumers count their tiles themselves —
-// exactly the round-1 loops.  Two instantiations rather than a run-time switch: with the switch the STATIC path of the transposing load ran
-// slower than the dedicated loops.
-template <bool DYN>
 __global__ void __launch_bounds__(kThreads, 1) kk_convert_kernel(const ConvertLaunch L) {
   extern __shared__ __align__(128) uint8_t smem[];
   uint8_t* stage_buf = smem;
@@ -279,7 +275,7 @@ __global__ void __launch_bounds__(kThreads, 1) kk_convert_kernel(const ConvertLa
       KKSeg seg = load_seg(L.segs);
       uint32_t it = 0;
       uint32_t tile = blockIdx.x, batch_next = 0, batch_left = 0;
-      uint32_t pre = DYN ? atomicAdd(L.sched, kBatch) : 0u;
+      uint32_t pre = atomicAdd(L.sched, kBatch);
       for (; tile < L.n_tiles; ++it) {
         const uint32_t s = it % kStages, ph = (it / kStages) & 1u;
         mbar_wait(empty0 + 8 * s, ph ^ 1u);
@@ -299,32 +295,26 @@ __global__ void __launch_bounds__(kThreads, 1) kk_convert_kernel(const ConvertLa
           else
             for (uint32_t r = 0; r < ld.nrows; ++r) bulk_g2s(sb + r * ld.spitch, L.src + ld.g_off + (uint64_t)r * ld.gpitch, ld.row_bytes, full0 + 8 * s);
         }
-        if (!DYN) {
-          tile += gridDim.x;
-        } else {
-          if (batch_left == 0) {
-            batch_next = gridDim.x + pre;
-            batch_left = kBatch;
-            pre = atomicAdd(L.sched, kBatch);
-          }
-          tile = batch_next++;
-          --batch_left;
+        if (batch_left == 0) {
+          batch_next = gridDim.x + pre;
+          batch_left = kBatch;
+          pre = atomicAdd(L.sched, kBatch);
         }
+        tile = batch_next++;
+        --batch_left;
       }
-      // end marker for the consumers (under dynamic draws they do not know their tile count in advance)
-      if (DYN) {
+      {  // end marker for the consumers, which do not know in advance how many tiles their CTA draws
         const uint32_t s = it % kStages, ph = (it / kStages) & 1u;
         mbar_wait(empty0 + 8 * s, ph ^ 1u);
         descs[s].op = KK_OP_END;
         mbar_arrive(full0 + 8 * s);
       }
-      if (DYN) {  // the last CTA to get here leaves the counters zeroed for the next launch on this stream
+      // the last CTA to get here leaves the counters zeroed for the next launch on this stream
+      __threadfence();
+      if (atomicAdd(L.sched + 1, 1u) == gridDim.x - 1u) {
+        L.sched[0] = 0u;
+        L.sched[1] = 0u;
         __threadfence();
-        if (atomicAdd(L.sched + 1, 1u) == gridDim.x - 1u) {
-          L.sched[0] = 0u;
-          L.sched[1] = 0u;
-          __threadfence();
-        }
       }
     }
   } else {
@@ -337,12 +327,11 @@ __global__ void __launch_bounds__(kThreads, 1) kk_convert_kernel(const ConvertLa
     D.multimem = (L.flags & KK_LAUNCH_MULTIMEM) != 0;
     D.single = (L.n_dst == 1) && !D.multimem;
     int pending = -1;  // stage whose bulk stores may still be reading shared memory (warp 1 lane 0 only)
-    uint32_t it = 0;
-    for (uint32_t tile = blockIdx.x; DYN || tile < L.n_tiles; tile += gridDim.x, ++it) {
+    for (uint32_t it = 0;; ++it) {
       const uint32_t s = it % kStages, ph = (it / kStages) & 1u;
       mbar_wait(full0 + 8 * s, ph);
       const TileDesc t = descs[s];
-      if (DYN && t.op == KK_OP_END) break;  // the producer's end marker
+      if (t.op == KK_OP_END) break;  // the producer's end marker
       const uint32_t sbase = smem_u32(stage_buf + s * kStageBytes);
       const uint32_t pay = sbase + t.pay_off;
       if (t.bulk == 1) {
@@ -504,18 +493,15 @@ __global__ void __launch_bounds__(256) kk_fill_kernel(uint4* __restrict__ dst, u
 }  // namespace
 
 cudaError_t kernels_init_device() {
-  cudaError_t e = cudaFuncSetAttribute(kk_convert_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kSmemFixed + 4 * kMaxSegsPerLaunch + 128));
-  if (e != cudaSuccess) return e;
-  return cudaFuncSetAttribute(kk_convert_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kSmemFixed + 4 * kMaxSegsPerLaunch + 128));
+  return cudaFuncSetAttribute(kk_convert_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kSmemFixed + 4 * kMaxSegsPerLaunch + 128));
 }
 
 cudaError_t launch_convert(const ConvertLaunch& L, int sm_count, cudaStream_t stream) {
   if (L.n_tiles == 0) return cudaSuccess;
-  if (L.n_segs == 0 || L.n_segs > kMaxSegsPerLaunch || L.n_dst == 0 || L.n_dst > KK_MAX_DST) return cudaErrorInvalidValue;
+  if (L.n_segs == 0 || L.n_segs > kMaxSegsPerLaunch || L.n_dst == 0 || L.n_dst > KK_MAX_DST || !L.sched) return cudaErrorInvalidValue;
   const uint32_t grid = L.n_tiles < (uint32_t)sm_count ? L.n_tiles : (uint32_t)sm_count;
   const size_t smem = kSmemFixed + 4 * (size_t)L.n_segs + 16;
-  if (L.sched) kk_convert_kernel<true><<<grid, kThreads, smem, stream>>>(L);
-  else kk_convert_kernel<false><<<grid, kThreads, smem, stream>>>(L);
+  kk_convert_kernel<<<grid, kThreads, smem, stream>>>(L);
   return cudaGetLastError();
 }
 

@@ -18,8 +18,8 @@ struct ConvertLaunch {
   uint8_t* xdst[KK_MAX_DST]; // KK_OP_ROWSPLIT only: pool of every rank, indexed by rank (all-to-all destinations)
   uint32_t n_xdst;
   uint32_t pad_;
-  // Dynamic tile scheduling: two zeroed uint32 in device memory, private to the STREAM this launch is enqueued on ([0] next batch of tiles,
-  // [1] CTAs finished; the last CTA zeroes both again, so consecutive launches on one stream share them).  nullptr: static round-robin.
+  // Tile-scheduling counters, required: two zeroed uint32 in device memory, private to the STREAM this launch is enqueued on ([0] next batch
+  // of tiles, [1] CTAs finished; the last CTA zeroes both again, so consecutive launches on one stream share them).
   uint32_t* sched;
 };
 

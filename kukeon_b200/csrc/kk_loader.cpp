@@ -275,18 +275,6 @@ void fill_raw_dsts(kk_model* m, int li, ConvertLaunch& L) {
   }
 }
 
-// Tile scheduling of a launch: dynamic (counters of the launching stream) for every plan.  On H100 this includes the transposing loads: the
-// GPT-2-small load takes 0.51 ms with dynamic draws against 0.70 ms under static round-robin (one H100 SXM, 700 W limit, 50 launches each,
-// twice, same build).  KUKEON_GPULOAD_SCHED=static forces static round-robin: a measurement knob for A/B runs of the two schedulers on one
-// box, not part of the API.
-uint32_t* sched_for(uint32_t* stream_counters) {
-  static const bool force_static = [] {
-    const char* e = getenv("KUKEON_GPULOAD_SCHED");
-    return e && !strcmp(e, "static");
-  }();
-  return force_static ? nullptr : stream_counters;
-}
-
 // Stream plan part `part` through the reader threads of local device `li`.  Each thread claims the next chunk, waits until its next slot's
 // previous work has run, reads the chunk into the pinned slot and calls consume(reader, slot, chunk index), which enqueues on the reader's
 // stream what moves the bytes on; the slot is free again once that has run.  record_times: this is the streaming pass of kk_load_part, whose
@@ -366,7 +354,7 @@ void convert_part(kk_model* m, int li, int part, const FdSet& fds) {
     L.segs = d_segs + ch.seg_begin;
     L.n_segs = ch.seg_count;
     L.n_tiles = ch.n_tiles;
-    L.sched = sched_for(rd.sched);
+    L.sched = rd.sched;
     KK_CUDA(launch_convert(L, sm_count, rd.stream));
   });
 }
@@ -391,7 +379,7 @@ void raw_stage1(kk_model* m, int li, const FdSet& fds) {
     L.segs = R.d_copy_segs + m->chunk_base[(size_t)part] + ci;
     L.n_segs = 1;
     L.n_tiles = (uint32_t)kk_seg_tiles(KK_OP_COPY, align_up(ch.buf_bytes, 16), 0);
-    L.sched = sched_for(rd.sched);
+    L.sched = rd.sched;
     KK_CUDA(launch_convert(L, sm_count, rd.stream));
   });
 }
@@ -475,7 +463,7 @@ float time_launches(kk_model* m, std::vector<std::vector<ConvertLaunch>>& launch
     evs[li].create_all();
     KK_CUDA(cudaEventRecord(evs[li][0], dev.stream));
     for (size_t k = 0; k < launches[li].size(); ++k) {
-      launches[li][k].sched = sched_for(dev.sched);
+      launches[li][k].sched = dev.sched;
       KK_CUDA(launch_convert(launches[li][k], dev.sm_count, dev.stream));
       KK_CUDA(cudaEventRecord(evs[li][k + 1], dev.stream));
     }

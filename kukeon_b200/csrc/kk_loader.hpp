@@ -32,7 +32,7 @@ struct Slot {
 
 struct Reader {
   cudaStream_t stream = nullptr;
-  uint32_t* sched = nullptr;  // two zeroed device words: the tile-scheduling counters of the launches on `stream` (ConvertLaunch::sched)
+  uint32_t* sched = nullptr;  // two zeroed device words: the tile-scheduling counters every launch on `stream` needs (ConvertLaunch::sched)
   std::vector<Slot> slots;
 };
 
@@ -44,7 +44,7 @@ struct Device {
   int sm_count = 0;
   std::vector<Reader> readers;
   cudaStream_t stream = nullptr;  // resident launches, checksum, misc
-  uint32_t* sched = nullptr;      // tile-scheduling counters of the launches on `stream` (first 8 of 256 zeroed bytes)
+  uint32_t* sched = nullptr;      // tile-scheduling counters every launch on `stream` needs (first 8 of 256 zeroed bytes)
   std::unique_ptr<std::mutex> sum_mu{new std::mutex};  // kk_checksum's accumulator is the 8 bytes at sched + 32 words: no cudaMalloc / cudaFree per call
   uint64_t pool_in_use = 0;
   bool kernels_ready = false;
