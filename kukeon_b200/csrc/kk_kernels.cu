@@ -357,16 +357,10 @@ __global__ void __launch_bounds__(kThreads, 1) kk_convert_kernel(const ConvertLa
         if (cwarp == 0) {
           if (lane == 0) {
             fence_proxy_async();
-            uint32_t pos = t.col0;
-            const uint32_t end = t.col0 + t.n_units;
-            uint32_t row = pos / t.C, col = pos - row * t.C;
-            while (pos < end) {
-              const uint32_t j = col / t.R, within = col - j * t.R;
-              uint32_t len = t.R - within;
-              if (len > end - pos) len = end - pos;
-              bulk_s2g(L.xdst[j] + t.dst_off + (uint64_t)(t.row0 + row) * t.R + within, pay + (pos - t.col0), len);
-              pos += len; col += len;
-              if (col >= t.C) { col = 0; ++row; }
+            for (KKRowSplitWalk w = kk_rowsplit_walk(t); w.pos < w.end;) {
+              const KKRowSplitPiece p = kk_rowsplit_piece(t, w);
+              bulk_s2g(L.xdst[p.dst.j] + p.dst.off, pay + p.src, p.len);
+              kk_rowsplit_advance(t, w, p.len);
             }
             bulk_commit();
             if (pending >= 0) {
@@ -393,10 +387,8 @@ __global__ void __launch_bounds__(kThreads, 1) kk_convert_kernel(const ConvertLa
       switch (t.op) {
         case KK_OP_ROWSPLIT: {  // unaligned fallback: byte-granular all-to-all copy
           for (uint32_t k = ctid; k < t.n_units; k += kConsumerThreads) {
-            const uint32_t pos = t.col0 + k;
-            const uint32_t row = pos / t.C, col = pos - row * t.C;
-            const uint32_t j = col / t.R, within = col - j * t.R;
-            L.xdst[j][t.dst_off + (uint64_t)(t.row0 + row) * t.R + within] = (uint8_t)lds8(pay + k);
+            const KKRowSplitDst x = kk_rowsplit_byte(t, k);
+            L.xdst[x.j][x.off] = (uint8_t)lds8(pay + k);
           }
           break;
         }

@@ -132,3 +132,67 @@ static inline KK_HD void kk_make_tile(const KKSeg& seg, uint32_t t, uint64_t src
       d.bulk = 3;
   }
 }
+
+// Row-split exchange (KK_OP_ROWSPLIT) addressing, shared by the kernel's two consumers and tests/emul.  A tile holds n_units bytes of this
+// rank's piece from byte col0 of it on; the piece is whole source rows of C bytes, tensor row row0 first.  Column `col` of piece row `row`
+// belongs to rank j = col / R and lands in that rank's pool at dst_off + (row0 + row) * R + col % R.
+struct KKRowSplitDst {
+  uint32_t j;       // destination rank (index into ConvertLaunch::xdst)
+  uint32_t within;  // column inside the rank's slice
+  uint64_t off;     // byte offset in that rank's pool
+};
+static inline KK_HD KKRowSplitDst kk_rowsplit_col(const KKTileDesc& d, uint32_t col) {  // rank and column in its slice; off is left 0
+  KKRowSplitDst x;
+  x.j = col / d.R;
+  x.within = col - x.j * d.R;
+  x.off = 0;
+  return x;
+}
+static inline KK_HD uint64_t kk_rowsplit_off(const KKTileDesc& d, uint32_t row, uint32_t within) {
+  return d.dst_off + (uint64_t)(d.row0 + row) * d.R + within;
+}
+
+// Byte k of the tile (the byte-granular consumer).
+static inline KK_HD KKRowSplitDst kk_rowsplit_byte(const KKTileDesc& d, uint32_t k) {
+  const uint32_t pos = d.col0 + k;
+  const uint32_t row = pos / d.C;
+  KKRowSplitDst x = kk_rowsplit_col(d, pos - row * d.C);
+  x.off = kk_rowsplit_off(d, row, x.within);
+  return x;
+}
+
+// The (row, destination rank) pieces of a tile, in order (the bulk-store consumer, t.bulk == 3): each piece is the longest run of the tile's
+// bytes inside one row and one slice.
+//   for (KKRowSplitWalk w = kk_rowsplit_walk(d); w.pos < w.end;) { p = kk_rowsplit_piece(d, w); <store p>; kk_rowsplit_advance(d, w, p.len); }
+struct KKRowSplitWalk {
+  uint32_t pos, end, row, col;  // byte position of the next piece in this rank's piece, end of the tile, the next piece's row and column
+};
+struct KKRowSplitPiece {
+  KKRowSplitDst dst;
+  uint32_t len;
+  uint32_t src;  // offset of the piece's first byte from the tile's payload
+};
+static inline KK_HD KKRowSplitWalk kk_rowsplit_walk(const KKTileDesc& d) {
+  KKRowSplitWalk w;
+  w.pos = d.col0;
+  w.end = d.col0 + d.n_units;
+  w.row = w.pos / d.C;
+  w.col = w.pos - w.row * d.C;
+  return w;
+}
+static inline KK_HD KKRowSplitPiece kk_rowsplit_piece(const KKTileDesc& d, const KKRowSplitWalk& w) {
+  KKRowSplitPiece p;
+  p.dst = kk_rowsplit_col(d, w.col);
+  p.len = d.R - p.dst.within;
+  if (p.len > w.end - w.pos) p.len = w.end - w.pos;
+  p.dst.off = kk_rowsplit_off(d, w.row, p.dst.within);
+  p.src = w.pos - d.col0;
+  return p;
+}
+static inline KK_HD void kk_rowsplit_advance(const KKTileDesc& d, KKRowSplitWalk& w, uint32_t len) {
+  w.pos += len;
+  w.col += len;
+  const bool wrap = w.col >= d.C;
+  w.row += wrap;
+  w.col = wrap ? 0u : w.col;
+}

@@ -501,14 +501,35 @@ extern "C" int kk_emul_t_tile(uint32_t op, const uint8_t* src, uint32_t C, uint3
   return g.err;
 }
 
+// A row-split store of `len` bytes into rank j's pool at `off`: the rank must have a pool, the bytes must lie inside it, and no byte of it may
+// have been stored before by any rank's launch.  Returns 0 or the failure code.
+static int rowsplit_store(uint8_t* const* xdst, uint32_t n_xdst, const uint64_t* xpool_bytes, uint8_t* const* xhits, uint8_t* const* xmask1,
+                          uint32_t j, uint64_t off, const uint8_t* v, uint32_t len) {
+  if (j >= n_xdst || !xdst[j]) return 17;
+  if (off > xpool_bytes[j] || len > xpool_bytes[j] - off) return 15;
+  for (uint32_t i = 0; i < len; ++i) {
+    if (xmask1[j][off + i]) return 4;
+    xmask1[j][off + i] = 1;
+    xhits[j][(off + i) >> 4] += 1;
+  }
+  memcpy(xdst[j] + off, v, len);
+  return 0;
+}
+
 // A whole launch of kk_convert_kernel, tile by tile: resolve the tile's segment from tile_begin[] (as the producer does), kk_make_tile (the
-// function the kernel's producer calls when built with KK_PRODUCER_SHARED), perform the bulk copies it asks for into a stage buffer with the
-// hardware's constraints checked (16-byte aligned source, destination and size; bytes issued == bytes announced), then the consumer side: the
-// aligned-copy bulk stores, or the same per-lane device functions the other entry points run, for all 16 x 32 consumer lanes.
+// function the kernel's producer calls), perform the bulk copies it asks for into a stage buffer with the hardware's constraints checked
+// (16-byte aligned source, destination and size; bytes issued == bytes announced), then the consumer side: the aligned-copy bulk stores, the
+// row-split exchange through the kernel's own addressing (kk_rowsplit_*), or the same per-lane device functions the other entry points run,
+// for all 16 x 32 consumer lanes.
 // src: the staged chunk (src base assumed 256-byte aligned like the staging buffers); dst[0..n_dst): destination pools of pool_bytes each;
-// hits / masks describe dst[0] and ACCUMULATE across calls (the caller zeroes them once per pool).  Not covered: the scatter row exchange (return -2).
+// hits / masks describe dst[0] and ACCUMULATE across calls (the caller zeroes them once per pool).
+// xdst[0..n_xdst): the pool of every rank, for KK_OP_ROWSPLIT tiles (ConvertLaunch::xdst); xpool_bytes, xhits and xmask1 are each pool's
+// size, 16-byte hit counters and per-byte store mask, shared with the launches of the other ranks so that a byte stored twice across ranks
+// fails.  rs_tiles (may be null) accumulates the row-split tiles played: [0] by bulk stores (bulk == 3), [1] by the byte-granular consumer.
 extern "C" int kk_emul_launch(const uint8_t* src, uint64_t src_bytes, const KKSeg* segs, uint32_t n_segs, uint32_t n_tiles, uint32_t flags,
-                              uint8_t* const* dst, uint32_t n_dst, uint64_t pool_bytes, uint8_t* hits, uint8_t* mask2, uint8_t* mask1) {
+                              uint8_t* const* dst, uint32_t n_dst, uint64_t pool_bytes, uint8_t* hits, uint8_t* mask2, uint8_t* mask1,
+                              uint8_t* const* xdst, uint32_t n_xdst, const uint64_t* xpool_bytes, uint8_t* const* xhits, uint8_t* const* xmask1,
+                              uint64_t* rs_tiles) {
   if (n_dst < 1 || n_dst > KK_MAX_DST) return -1;
   static thread_local uint8_t stage[KK_TILE_SRC_BYTES + KK_STAGE_PAD];
   const uint64_t src_addr = 0x100000;  // only the alignment of the src base matters
@@ -559,7 +580,28 @@ extern "C" int kk_emul_launch(const uint8_t* src, uint64_t src_bytes, const KKSe
       for (uint32_t i = 0; i < n_dst; ++i) memcpy(dst[i] + d.dst_off, stage + d.pay_off, d.n_units);
       continue;
     }
-    if (d.bulk == 3 || d.op == KK_OP_ROWSPLIT) return -2;
+    if (d.op == KK_OP_ROWSPLIT) {
+      if (!d.C || !d.R) return 18;  // the kernel would divide by zero
+      if (d.bulk == 3) {  // one bulk store per (row, rank) piece, from warp 0 lane 0
+        for (KKRowSplitWalk w = kk_rowsplit_walk(d); w.pos < w.end;) {
+          const KKRowSplitPiece p = kk_rowsplit_piece(d, w);
+          const uint32_t s0 = d.pay_off + p.src;
+          if ((p.dst.off & 15u) || (s0 & 15u) || (p.len & 15u) || !p.len) return 14;
+          if (s0 + p.len > staged) return 16;
+          if (int rc = rowsplit_store(xdst, n_xdst, xpool_bytes, xhits, xmask1, p.dst.j, p.dst.off, stage + s0, p.len)) return rc;
+          kk_rowsplit_advance(d, w, p.len);
+        }
+      } else {  // byte-granular consumer: every consumer thread strides over the tile
+        for (int t = 0; t < kConsumerThreads; ++t)
+          for (uint32_t k = (uint32_t)t; k < d.n_units; k += kConsumerThreads) {
+            const KKRowSplitDst x = kk_rowsplit_byte(d, k);
+            if (d.pay_off + k >= staged) return 16;
+            if (int rc = rowsplit_store(xdst, n_xdst, xpool_bytes, xhits, xmask1, x.j, x.off, stage + d.pay_off + k, 1)) return rc;
+          }
+      }
+      if (rs_tiles) ++rs_tiles[d.bulk == 3 ? 0 : 1];
+      continue;
+    }
     switch (d.op) {
       case KK_OP_T_F32_BF16: case KK_OP_T_F16_BF16: case KK_OP_T_B16: case KK_OP_T_B32: {
         const uint32_t es = kk_t_src_es(d.op);

@@ -128,6 +128,37 @@ def emulate_part(plan: dict, part: int, pool_bytes: int, exchange: dict | None =
     return pool, mask
 
 
+def rowsplit_tile_classes(plan: dict) -> Tuple[int, int]:
+    """(bulk-store tiles, byte-granular tiles) of every KK_OP_ROWSPLIT segment of every part: kk_make_tile's condition for bulk == 3,
+    with the chunk's base 16-byte aligned as the staging buffers and the resident image are."""
+    T = 32768
+    bulk = fallback = 0
+    for part in plan["parts"]:
+        for ch in part["chunks"]:
+            for sg in ch["segs"]:
+                if sg["op"] != OP_ROWSPLIT:
+                    continue
+                for o in range(0, sg["units"], T):
+                    n = min(T, sg["units"] - o)
+                    if (sg["src_off"] + o) % 16 == 0 and sg["p0"] % 16 == 0 and sg["p1"] % 16 == 0 and n % 16 == 0 and sg["dst_off"] % 16 == 0:
+                        bulk += 1
+                    else:
+                        fallback += 1
+    return bulk, fallback
+
+
+# Row-parallel tensors whose row-split exchange leaves the aligned bulk path: a 7-element norm first (14 bytes, so everything after it sits off
+# 16 in an unpadded file), slices that are no multiple of 16 bytes, verbatim U8 / FP8, rows longer than a tile (57 KB) and a tensor with
+# fewer rows (5) than there are ranks at n = 8.
+ROWSPLIT_ODD_TENSORS = [("model.layers.0.input_layernorm.weight", "BF16", [7]),
+                        ("model.layers.0.self_attn.o_proj.weight", "BF16", [100, 120]),
+                        ("model.layers.0.mlp.down_proj.weight", "BF16", [67, 3000]),
+                        ("model.layers.1.mlp.down_proj.weight", "U8", [33, 840]),
+                        ("model.layers.1.self_attn.o_proj.weight", "F8_E4M3", [129, 360]),
+                        ("model.layers.2.mlp.down_proj.weight", "BF16", [40, 28672]),
+                        ("model.layers.2.self_attn.o_proj.weight", "BF16", [5, 16])]
+
+
 def expected_mask(plan_pool: List[dict], total: int) -> np.ndarray:
     m = np.zeros(total, bool)
     for p in plan_pool:

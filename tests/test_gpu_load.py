@@ -603,39 +603,61 @@ def test_virtual_ranks_broadcast_on_one_gpu(pool, tmp_path, n):
                 m.release()
 
 
-@pytest.mark.parametrize("n", [2, 4, 8])
-def test_virtual_ranks_scatter_exchange_on_one_gpu(pool, tmp_path, n):
-    """KK_LOAD_SCATTER_EXCHANGE: rank i ingests whole rows of the row-parallel tensors and the KK_OP_ROWSPLIT tiles deal
-    every row's column slices to the n pools; every rank's pool must equal its oracle slice pool."""
-    d = str(tmp_path / "llama")
-    synth.make_llama(d, dict(hidden=512, ffn=1408, layers=2, kv_dim=128, vocab=2048), max_shard_bytes=6_000_000)
-    shards, recs = oracle.index_path(d)
-    for flags in (gpupool.LOAD_SCATTER_EXCHANGE, 0):
-        ms = _virtual_ranks(pool, d, gpupool.MODE_SCATTER, n, flags)
-        try:
+def _exchange_on_virtual_ranks(pool, path, n, shards, recs, flags):
+    ms = _virtual_ranks(pool, path, gpupool.MODE_SCATTER, n, flags)
+    try:
+        for m in ms:
+            m.load_part()
+        for i, m in enumerate(ms):
+            assert_pool_matches(m, 0, shards, recs, mode=gpupool.MODE_SCATTER, n_parts=n, part=i)
+        if flags:
             for m in ms:
-                m.load_part()
+                m.stage_resident()
+            for m in ms:
+                m.convert_resident()
             for i, m in enumerate(ms):
                 assert_pool_matches(m, 0, shards, recs, mode=gpupool.MODE_SCATTER, n_parts=n, part=i)
-            if flags:
-                for m in ms:
-                    m.stage_resident()
-                for m in ms:
-                    m.convert_resident()
-                for i, m in enumerate(ms):
-                    assert_pool_matches(m, 0, shards, recs, mode=gpupool.MODE_SCATTER, n_parts=n, part=i)
-                st = ms[0].stats()
-                assert st["local_src_bytes"] < st["file_bytes"] / n * 1.1 + (1 << 20)
-        finally:
-            for m in ms:
-                m.release()
-    # without the peers attached an exchange load must refuse, not silently drop the slices of other ranks
-    m = pool.load(d, mode=gpupool.MODE_SCATTER, flags=gpupool.LOAD_SCATTER_EXCHANGE | gpupool.LOAD_DEFER, part_index=0, part_count=n)
-    try:
-        with pytest.raises(gpupool.ErrState, match="not reachable"):
-            m.load_part()
+        return [m.stats() for m in ms]
     finally:
-        m.release()
+        for m in ms:
+            m.release()
+
+
+@pytest.mark.parametrize("n", [2, 3, 4, 5, 8])
+def test_virtual_ranks_scatter_exchange_on_one_gpu(pool, tmp_path, n):
+    """KK_LOAD_SCATTER_EXCHANGE: rank i ingests whole rows of the row-parallel tensors and the KK_OP_ROWSPLIT tiles deal
+    every row's column slices to the n pools; every rank's pool must equal its oracle slice pool, after the streaming load and
+    again after the resident conversion.  Llama shapes at n = 2, 4, 8 (every tile on the bulk-store pieces); at n = 2, 3, 5, 8 a file
+    of odd shapes, padded and unpadded, whose tiles take both the bulk-store pieces and the byte-granular consumer, through a pool of
+    small staging buffers."""
+    X = gpupool.LOAD_SCATTER_EXCHANGE
+    if n in (2, 4, 8):
+        d = str(tmp_path / "llama")
+        synth.make_llama(d, dict(hidden=512, ffn=1408, layers=2, kv_dim=128, vocab=2048), max_shard_bytes=6_000_000)
+        shards, recs = oracle.index_path(d)
+        for flags in (X, 0):
+            stats = _exchange_on_virtual_ranks(pool, d, n, shards, recs, flags)
+            if flags:
+                assert stats[0]["local_src_bytes"] < stats[0]["file_bytes"] / n * 1.1 + (1 << 20)
+        # without the peers attached an exchange load must refuse, not silently drop the slices of other ranks
+        m = pool.load(d, mode=gpupool.MODE_SCATTER, flags=X | gpupool.LOAD_DEFER, part_index=0, part_count=n)
+        try:
+            with pytest.raises(gpupool.ErrState, match="not reachable"):
+                m.load_part()
+        finally:
+            m.release()
+    if n in (2, 3, 5, 8):
+        with gpupool.Pool([0], n_staging_buffers=2, staging_buffer_bytes=1 * MB, n_reader_threads=1) as small:
+            for pad in (True, False):
+                p = str(tmp_path / f"odd{int(pad)}.safetensors")
+                synth.write_safetensors(p, helpers.ROWSPLIT_ODD_TENSORS, 3, pad_header=pad)
+                shards, recs = oracle.index_path(p)
+                stats = _exchange_on_virtual_ranks(small, p, n, shards, recs, X)
+                plan = gpupool.plan_describe(p, mode=gpupool.MODE_SCATTER, flags=X, n_parts=n, chunk_bytes=2 * MB)  # staging slots are whole 2 MiB
+                ran = [next((q["chunks"], q["tiles"]) for q in st["parts"] if q["part"] == i) for i, st in enumerate(stats)]
+                assert ran == [(len(q["chunks"]), sum(ch["n_tiles"] for ch in q["chunks"])) for q in plan["parts"]], "the load ran another plan"
+                bulk, fallback = helpers.rowsplit_tile_classes(plan)
+                assert bulk > 0 and fallback > 0, (bulk, fallback)
 
 
 def test_concurrent_loads_of_different_checkpoints_share_the_staging_ring_safely(pool, tmp_path):

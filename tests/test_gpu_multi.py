@@ -10,6 +10,7 @@ import torch
 
 from kukeon_b200 import gpupool
 from oracle import oracle
+from tests import helpers
 from tools import synth
 
 pytestmark = [pytest.mark.gpu, pytest.mark.multigpu]
@@ -110,17 +111,21 @@ def test_single_process_scatter(native, tmp_path):
 
 @needs2
 def test_single_process_scatter_exchange(native, tmp_path):
+    """Llama shapes, then a file of odd shapes whose row-split tiles also take the byte-granular consumer."""
     n = min(_ngpu(), 8)
     d = str(tmp_path / "llama")
     synth.make_llama(d, dict(hidden=512, ffn=1408, layers=2, kv_dim=128, vocab=2048), max_shard_bytes=6_000_000)
-    shards, recs = oracle.index_path(d)
+    q = str(tmp_path / "odd.safetensors")
+    synth.write_safetensors(q, helpers.ROWSPLIT_ODD_TENSORS, 3, pad_header=False)
     with gpupool.Pool(list(range(n)), n_staging_buffers=2, staging_buffer_bytes=1 * MB, n_reader_threads=1) as pl:
-        m = pl.load(d, mode=gpupool.MODE_SCATTER, flags=gpupool.LOAD_SCATTER_EXCHANGE)
-        try:
-            for dev in range(n):
-                check_pool(m, dev, shards, recs, mode=gpupool.MODE_SCATTER, n_parts=n, part=dev)
-        finally:
-            m.release()
+        for path in (d, q):
+            shards, recs = oracle.index_path(path)
+            m = pl.load(path, mode=gpupool.MODE_SCATTER, flags=gpupool.LOAD_SCATTER_EXCHANGE)
+            try:
+                for dev in range(n):
+                    check_pool(m, dev, shards, recs, mode=gpupool.MODE_SCATTER, n_parts=n, part=dev)
+            finally:
+                m.release()
 
 
 def _free_port():

@@ -2,12 +2,13 @@
 
 For every staged chunk the planner produces (kk_plan_describe), the chunk buffer is filled as the reader threads would fill it and the
 launch is played tile by tile: segment lookup from tile_begin[], `kk_make_tile` (csrc/kk_tile.h — the function the kernel's producer warp
-calls in the KK_PRODUCER_SHARED build), the bulk copies it asks for with the TMA constraints checked, then the consumer code of
-csrc/kk_consume_core.cuh / kk_dequant.cuh for all 16 x 32 lanes, storing into every destination pool of the launch.  The pools must equal
-the oracle's, every pool byte a tensor owns must have been stored exactly once, and nothing else may have been touched.
+calls), the bulk copies it asks for with the TMA constraints checked, then the consumer code of csrc/kk_consume_core.cuh / kk_dequant.cuh
+for all 16 x 32 lanes, storing into every destination pool of the launch.  The scatter row exchange (KK_OP_ROWSPLIT) is played through the
+kernel's own row-split addressing (kk_rowsplit_* in kk_tile.h): every rank's launch stores into all ranks' pools, its bulk-store pieces with
+their 16-byte alignment checked.  The pools must equal the oracle's, every pool byte a tensor owns must have been stored exactly once across
+all launches, and nothing else may have been touched.
 
-Not covered here (GPU tests only): the 32x128 transposes and the scatter row exchange (their consumer code still lives in kk_kernels.cu),
-mbarrier / proxy-fence protocol, anything about timing."""
+Not covered here (GPU tests only): the mbarrier / proxy-fence protocol and anything about timing."""
 import ctypes as C
 import os
 import subprocess
@@ -26,7 +27,9 @@ MB = 1 << 20
 ERR = {1: "shared load outside the staged bytes", 2: "misaligned shared load", 3: "store outside the pool / misaligned", 4: "pool bytes stored twice",
        8: "codebook index out of range", 9: "tile_begin[] not monotone", 10: "bulk copy violates 16-byte alignment / size / stage capacity",
        11: "bulk copy reads outside the staged chunk", 12: "bytes issued != bytes announced to the mbarrier", 13: "bulk store misaligned or outside the pool",
-       -1: "op not covered by the emulator", -2: "op whose consumer still lives in kk_kernels.cu"}
+       14: "row-split bulk piece: destination, stage offset or length not 16-byte aligned", 15: "row-split store outside the destination pool",
+       16: "row-split store reads outside the staged bytes", 17: "row-split store to a rank without a pool", 18: "row-split tile with zero row or slice bytes",
+       -1: "op not covered by the emulator"}
 
 
 class KKSeg(C.Structure):
@@ -39,7 +42,8 @@ def emul():
     subprocess.run(["make", "-C", os.path.join(_HERE, "emul"), "-s"], check=True)
     L = C.CDLL(os.environ.get("KK_EMUL_LIB") or os.path.join(_HERE, "emul", "_build", "libkk_dequant_emul.so"))  # override: A/B variants below
     L.kk_emul_launch.argtypes = [C.c_void_p, C.c_uint64, C.POINTER(KKSeg), C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(C.c_void_p), C.c_uint32, C.c_uint64,
-                                 C.c_void_p, C.c_void_p, C.c_void_p]
+                                 C.c_void_p, C.c_void_p, C.c_void_p,
+                                 C.POINTER(C.c_void_p), C.c_uint32, C.POINTER(C.c_uint64), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_uint64)]
     L.kk_emul_launch.restype = C.c_int
     assert C.sizeof(KKSeg) == 48
     return L
@@ -54,7 +58,20 @@ class Pools:
         self.ptrs = (C.c_void_p * n)(*[b.ctypes.data for b in self.bufs])
 
 
-def play_part(L, plan, part, pools, flags=0):
+class Exchange:
+    """The pools of all ranks as a row-split launch sees them (ConvertLaunch::xdst), with each pool's hit counters and byte mask, and the
+    row-split tiles played so far: tiles[0] by bulk stores, tiles[1] by the byte-granular consumer."""
+    def __init__(self, ranks):
+        n = len(ranks)
+        self.args = ((C.c_void_p * n)(*[r.bufs[0].ctypes.data for r in ranks]), n, (C.c_uint64 * n)(*[r.bufs[0].size for r in ranks]),
+                     (C.c_void_p * n)(*[r.hits.ctypes.data for r in ranks]), (C.c_void_p * n)(*[r.m1.ctypes.data for r in ranks]))
+        self.tiles = (C.c_uint64 * 2)()
+
+
+NO_EXCHANGE = (None, 0, None, None, None)
+
+
+def play_part(L, plan, part, pools, flags=0, x=None):
     fhs = [open(s, "rb") for s in plan["shards"]]
     try:
         for ch in plan["parts"][part]["chunks"]:
@@ -65,7 +82,7 @@ def play_part(L, plan, part, pools, flags=0):
             segs = (KKSeg * len(ch["segs"]))(*[KKSeg(s["src_off"], s["dst_off"], s["units"], s["op"], s["tile_begin"], s["p0"], s["p1"], s["p2"], s["p3"])
                                               for s in ch["segs"]])
             rc = L.kk_emul_launch(buf.ctypes.data, buf.size, segs, len(ch["segs"]), ch["n_tiles"], flags, pools.ptrs, len(pools.bufs), pools.bufs[0].size,
-                                  pools.hits.ctypes.data, pools.m2.ctypes.data, pools.m1.ctypes.data)
+                                  pools.hits.ctypes.data, pools.m2.ctypes.data, pools.m1.ctypes.data, *(x.args if x else NO_EXCHANGE), x.tiles if x else None)
             assert rc == 0, f"part {part}: {ERR.get(rc, rc)}"
     finally:
         for fh in fhs:
@@ -81,23 +98,28 @@ def check(pools, exp, pl):
         assert (b[~mask] == 0xCD).all(), f"pool {k}: bytes outside every tensor were written"
 
 
-def replay(L, path, mode=gpupool.MODE_SINGLE, flags=0, n_parts=1, chunk=1 * MB):
+def replay(L, path, mode=gpupool.MODE_SINGLE, flags=0, n_parts=1, chunk=1 * MB, plan=None):
+    """Replay every part of the plan (or of `plan`, when given) and check the pools.  Returns the plan and the row-split tiles played
+    (bulk-store, byte-granular)."""
     shards, recs = oracle.index_path(path)
-    plan = gpupool.plan_describe(path, mode=mode, flags=flags, n_parts=n_parts, chunk_bytes=chunk)
+    plan = plan or gpupool.plan_describe(path, mode=mode, flags=flags, n_parts=n_parts, chunk_bytes=chunk)
     oflags = flags & (1 | 2 | 16)
+    x = None
     if mode == gpupool.MODE_SCATTER:
+        exps = [oracle.expected_pool(shards, recs, mode, oflags, n_parts, g) for g in range(n_parts)]
+        ranks = [Pools(1, len(exp)) for exp, _ in exps]
+        x = Exchange(ranks)  # every rank's launch may store into every rank's pool: the row exchange
         for g in range(n_parts):
-            exp, pl = oracle.expected_pool(shards, recs, mode, oflags, n_parts, g)
-            pools = Pools(1, len(exp))
-            play_part(L, plan, g, pools)
-            check(pools, exp, pl)
+            play_part(L, plan, g, ranks[g], x=x)
+        for g in range(n_parts):
+            check(ranks[g], *exps[g])
     else:
         exp, pl = oracle.expected_pool(shards, recs, mode, oflags)
         pools = Pools(n_parts, len(exp))  # every rank's launch stores into all N pools (the fused fan-out)
         for g in range(n_parts):
             play_part(L, plan, g, pools)
         check(pools, exp, pl)
-    return plan
+    return plan, (tuple(x.tiles) if x else (0, 0))
 
 
 def test_llama_bf16_bulk_store_path_single_broadcast_scatter(emul, tmp_path):
@@ -147,17 +169,55 @@ def test_transpose_tiles_through_whole_launches(emul, tmp_path):
                        ("F32", 41, True), ("F16", 43, True)):
         p = str(tmp_path / f"gpt2_{dt}_{d}_{int(pad)}.safetensors")
         synth.write_safetensors(p, [("x", "U8", [3])] + synth.gpt2_tensors(n_layer=1, d=d, vocab=50, n_pos=8, dtype=dt), 3, pad_header=pad)
-        plan = replay(emul, p, flags=T)
+        plan, _ = replay(emul, p, flags=T)
         assert {sg["op"] for ch in plan["parts"][0]["chunks"] for sg in ch["segs"]} & tr
     # rows wider than one tile: 3096 and 4128 columns are cut into equal pieces (a whole d = 1032 layer is 50 MB of pools and hit maps; 72 rows of it do)
     p = str(tmp_path / "gpt2_wide.safetensors")
     synth.write_safetensors(p, [("h.0.attn.c_attn.weight", "F32", [72, 3096]), ("h.0.mlp.c_fc.weight", "F32", [72, 4128]), ("h.0.mlp.c_proj.weight", "F16", [4128, 72])], 3)
-    plan = replay(emul, p, flags=T)
+    plan, _ = replay(emul, p, flags=T)
     assert {sg["op"] for ch in plan["parts"][0]["chunks"] for sg in ch["segs"]} & tr
     p = str(tmp_path / "gpt2_b.safetensors")
     synth.make_gpt2(p, n_layer=2, d=96, vocab=301, n_pos=40)
     replay(emul, p, flags=T, mode=gpupool.MODE_BROADCAST, n_parts=3)
     replay(emul, p, flags=T | gpupool.LOAD_KEEP_F32)
+
+
+def test_scatter_row_exchange_through_whole_launches(emul, tmp_path):
+    """KK_LOAD_SCATTER_EXCHANGE, every rank replayed: the ROWSPLIT tiles of rank i deal every row's column slices to all n pools, through
+    the bulk-store pieces (bulk == 3) where the geometry is 16-byte aligned and the byte-granular consumer elsewhere.  Llama shapes (all
+    aligned), then a file of odd shapes padded and unpadded at n = 2..8, with 1 MB chunks and the smallest the planner accepts (64 KB), which
+    split pieces mid-row.  The tiles of each class that ran must be those the plan calls for, and both classes must run where the shapes ask."""
+    X = gpupool.LOAD_SCATTER_EXCHANGE
+    d = str(tmp_path / "llama")
+    synth.make_llama(d, dict(hidden=512, ffn=1408, layers=2, kv_dim=128, vocab=2048), max_shard_bytes=6_000_000)
+    for n in (2, 4, 8):
+        for chunk in (8 * MB, 64 * 1024):
+            plan, tiles = replay(emul, d, mode=gpupool.MODE_SCATTER, flags=X, n_parts=n, chunk=chunk)
+            assert tiles == helpers.rowsplit_tile_classes(plan) and tiles[0] > 0, (n, chunk, tiles)
+    for pad in (True, False):
+        p = str(tmp_path / f"odd{int(pad)}.safetensors")
+        synth.write_safetensors(p, helpers.ROWSPLIT_ODD_TENSORS, 3, pad_header=pad)
+        for n in (2, 3, 4, 5, 6, 8):
+            for chunk in (1 * MB, 64 * 1024):
+                plan, tiles = replay(emul, p, mode=gpupool.MODE_SCATTER, flags=X, n_parts=n, chunk=chunk)
+                assert tiles == helpers.rowsplit_tile_classes(plan), (pad, n, chunk, tiles)
+                assert tiles[1] > 0 and (tiles[0] > 0 or n == 6), (pad, n, chunk, tiles)  # n = 6: no slice is a multiple of 16 bytes
+                if chunk < MB:
+                    assert any(sg["op"] == helpers.OP_ROWSPLIT and sg["p3"] % sg["p0"] for part in plan["parts"] for ch in part["chunks"] for sg in ch["segs"])
+
+
+def test_the_replay_notices_a_wrong_row_split_plan(emul, tmp_path):
+    """Liveness of the exchange replay: a ROWSPLIT segment with a wrong slice width (p1) or first row (p2) must fail it."""
+    p = str(tmp_path / "odd.safetensors")
+    synth.write_safetensors(p, helpers.ROWSPLIT_ODD_TENSORS, 3)
+    X, n = gpupool.LOAD_SCATTER_EXCHANGE, 4
+    for field, delta in (("p1", 16), ("p1", -16), ("p2", 1), ("p2", -1)):
+        for bulk in (True, False):  # a segment with 16-byte slices (bulk-store pieces), and one without (the byte-granular consumer)
+            plan = gpupool.plan_describe(p, mode=gpupool.MODE_SCATTER, flags=X, n_parts=n, chunk_bytes=1 * MB)
+            segs = [sg for sg in plan["parts"][1]["chunks"][0]["segs"] if sg["op"] == helpers.OP_ROWSPLIT and (sg["p1"] % 16 == 0) == bulk and sg["p2"] > 0]
+            segs[0][field] += delta
+            with pytest.raises(AssertionError):
+                replay(emul, p, mode=gpupool.MODE_SCATTER, flags=X, n_parts=n, plan=plan)
 
 
 def test_the_replay_notices_a_wrong_plan(emul, tmp_path):
@@ -175,10 +235,10 @@ def test_the_replay_notices_a_wrong_plan(emul, tmp_path):
     s = ch["segs"][0]
     seg = (KKSeg * 1)(KKSeg(s["src_off"], s["dst_off"], s["units"], s["op"], 1, 0, 0, 0, 0))  # first tile has no segment
     pools = Pools(1, len(exp))
-    assert emul.kk_emul_launch(buf.ctypes.data, buf.size, seg, 1, ch["n_tiles"], 0, pools.ptrs, 1, len(exp), pools.hits.ctypes.data, pools.m2.ctypes.data, pools.m1.ctypes.data) == 9
+    assert emul.kk_emul_launch(buf.ctypes.data, buf.size, seg, 1, ch["n_tiles"], 0, pools.ptrs, 1, len(exp), pools.hits.ctypes.data, pools.m2.ctypes.data, pools.m1.ctypes.data, *NO_EXCHANGE, None) == 9
     seg = (KKSeg * 1)(KKSeg(s["src_off"], s["dst_off"], s["units"], s["op"], 0, 0, 0, 0, 0))
     pools = Pools(1, len(exp))
-    assert emul.kk_emul_launch(buf.ctypes.data, buf.size // 2, seg, 1, ch["n_tiles"], 0, pools.ptrs, 1, len(exp), pools.hits.ctypes.data, pools.m2.ctypes.data, pools.m1.ctypes.data) == 11
+    assert emul.kk_emul_launch(buf.ctypes.data, buf.size // 2, seg, 1, ch["n_tiles"], 0, pools.ptrs, 1, len(exp), pools.hits.ctypes.data, pools.m2.ctypes.data, pools.m1.ctypes.data, *NO_EXCHANGE, None) == 11
 
 
 # ---- property tests: random inventories through whole launches of the device code ---------------------------------------------------------
@@ -189,7 +249,7 @@ from tests.test_plan_property import gguf_inventories, inventories  # noqa: E402
 
 @settings(max_examples=int(os.environ.get("KK_HYP_EXAMPLES", 120)), deadline=None, suppress_health_check=[HealthCheck.too_slow, HealthCheck.function_scoped_fixture])
 @given(inv=inventories(), mode=st.sampled_from([0, 1, 2]), n_parts=st.integers(1, 6), pad=st.booleans(),
-       flags=st.sampled_from([0, 2, 16, 18, 33, 35, 49, 65, 67, 81]))  # every flag set whose ops the replay covers (no 32x128 transposes, no row exchange)
+       flags=st.sampled_from([0, 2, 16, 18, 33, 35, 49, 65, 67, 81, 8, 10, 24, 26, 41, 43, 57, 73, 75, 89]))  # each set also with the row exchange (8)
 def test_random_safetensors_inventories_replayed_through_the_device_code(emul, inv, mode, n_parts, pad, flags):
     import tempfile
     if mode == 0:
@@ -197,10 +257,6 @@ def test_random_safetensors_inventories_replayed_through_the_device_code(emul, i
     with tempfile.TemporaryDirectory() as d:
         p = os.path.join(d, "m.safetensors")
         synth.write_safetensors(p, inv, seed=7, pad_header=pad)
-        plan = gpupool.plan_describe(p, mode=mode, flags=flags, n_parts=n_parts, chunk_bytes=1 * MB)
-        ops = {sg["op"] for part in plan["parts"] for ch in part["chunks"] for sg in ch["segs"]}
-        if ops & {helpers.OP_T_F32_BF16, helpers.OP_T_F16_BF16, helpers.OP_T_B16, helpers.OP_T_B32, helpers.OP_ROWSPLIT}:
-            return  # R % 8 != 0 or 4-byte outputs keep the 32x128 ops, whose consumer is not in the shared headers
         replay(emul, p, mode=mode, flags=flags, n_parts=n_parts)
 
 
