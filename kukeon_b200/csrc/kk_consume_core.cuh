@@ -1,8 +1,8 @@
 // Core consumer bodies of kk_convert_kernel: verbatim copy (register path), fp32 / fp16 -> bf16 casts and the Q4_K dequantiser.
 // Like kk_dequant.cuh this file is written from the point of view of one lane against primitives the including translation
-// unit binds (see the list at the top of kk_dequant.cuh; additionally lds64, store1_all, kk_h2x2f, kConsumerThreads and — for
-// Q4_K, the one function here whose lanes trade values — __shfl_sync): PTX in kk_kernels.cu, checked C++ in
-// tests/emul/kk_dequant_emul.cpp, where the warp shuffle is emulated by running each warp twice (record, then replay).
+// unit binds (see the list at the top of kk_dequant.cuh; additionally lds64, store1_all, kk_h2x2f and — for Q4_K, the one
+// function here whose lanes trade values — __shfl_sync): PTX in kk_kernels.cu, checked C++ in tests/emul/kk_dequant_emul.cpp,
+// where the warp shuffle is emulated by playing every tile twice (record, then replay).
 #pragma once
 #include "kk_ops.h"
 

@@ -22,10 +22,13 @@
 //     uint64_t kk_grid_iq2xxs/iq2xs/iq2s/iq1s(i), uint32_t kk_grid_iq3xxs/iq3s(i)   codebook entry i (kk_iq_grids.h; __ldg on the device)
 //     void     sts16(a, v) / sts32(a, v)         stores into the stage (gather fallback of the 8-row transposes)
 //     uint32_t kk_ldg8(p)                        one byte from global memory (same fallback)
-//     Dsts, uint4, make_uint4, kConsumerWarps, KK_DQ_DEV (function attributes)
+//     void     named_bar_consumers()             barrier of the consumer threads (between that gather and its consumers)
+//     void     rowsplit_store1(L, j, off, v)     one byte into rank j's pool at off (row-split fallback; L: the launch, L.xdst on the device)
+//     Dsts, uint4, make_uint4, kConsumerWarps, kConsumerThreads, KK_DQ_DEV (function attributes)
 // kk_kernels.cu binds them to PTX; tests/emul/kk_dequant_emul.cpp binds them to plain C++ (with alignment and
-// write-once checks) and runs all 16 x 32 lanes in a loop, so the lane -> element index arithmetic of exactly this source
-// is checked against the oracle on the CPU test tier.  That harness is test infrastructure: the product has no CPU path.
+// write-once checks) and plays all 16 x 32 lanes of a tile through kk_consume_tile (kk_consume_tile.cuh), so the lane -> element
+// index arithmetic of exactly this source is checked against the oracle on the CPU test tier.  That harness is test infrastructure:
+// the product has no CPU path.
 //
 // Lane mapping of the dequantisers, same for every type: a lane produces 8 consecutive weights = one 16-byte bf16 store; a warp
 // iteration produces 512 contiguous output bytes (256-weight super-blocks: one block; 32-weight blocks: eight blocks).

@@ -16,6 +16,8 @@
 //       2-D transposes    : 8-row tiles staged by bulk copies, thread = column, one 16-byte store per column (GPT-2 Conv1D weights).
 //   Every output vector is stored to n_dst pools; dst[1..] are NVLink peer mappings, so conversion and
 //   broadcast are ONE kernel and the source bytes are read from HBM exactly once.
+//   The consumer loop keeps the stage protocol and the two bulk-store paths; every other tile goes through kk_consume_tile
+//   (kk_consume_tile.cuh), the dispatch tests/emul plays on the CPU.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
@@ -28,7 +30,7 @@ namespace kk {
 namespace {
 
 constexpr int kStages = 4;
-constexpr int kConsumerWarps = 16;  // 16 rather than 8: faster q4_K and much faster transposes; 20 (80 registers) is no faster
+constexpr int kConsumerWarps = KK_CONSUMER_WARPS;
 constexpr int kConsumerThreads = kConsumerWarps * 32;
 constexpr int kThreads = 32 + kConsumerThreads;  // 544
 constexpr uint32_t kStageBytes = KK_TILE_SRC_BYTES + KK_STAGE_PAD;
@@ -102,6 +104,7 @@ __device__ __forceinline__ void stmm128(void* p, const uint4& v) {  // NVLS mult
                : "memory");
 }
 __device__ __forceinline__ void named_bar_consumers() { asm volatile("bar.sync 1, %0;" ::"n"(kConsumerThreads) : "memory"); }
+__device__ __forceinline__ void rowsplit_store1(const ConvertLaunch& L, uint32_t j, uint64_t off, uint8_t v) { L.xdst[j][off] = v; }
 
 // Two floats -> packed bf16x2 (a in the low half), round-to-nearest-even; NaN -> 0x7FFF.
 __device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
@@ -169,7 +172,8 @@ __device__ __forceinline__ void store4_all(const Dsts& D, uint64_t off, uint32_t
 
 // ---- consumer bodies ------------------------------------------------------------------------------------------------------------
 // Every per-lane consumer function lives in kk_consume_core.cuh (copy, casts, Q4_K) and kk_dequant.cuh (the other block types, FP8,
-// 8-row transposes), written against the primitives bound here so that tests/emul can compile the same source for the host.
+// 8-row transposes), and the per-tile dispatch between them in kk_consume_tile.cuh, all written against the primitives bound here so
+// that tests/emul can compile the same source for the host.
 __device__ __forceinline__ uint32_t lds16(uint32_t a) { return lds_plain<uint16_t>(a); }
 __device__ __forceinline__ uint32_t lds32(uint32_t a) { return lds_plain<uint32_t>(a); }
 __device__ __forceinline__ float kk_h2f(uint32_t h) { return __half2float(__ushort_as_half((unsigned short)h)); }
@@ -214,21 +218,7 @@ __device__ __forceinline__ uint32_t kk_grid_iq3xxs(uint32_t i) { return __ldg(&k
 __device__ __forceinline__ uint32_t kk_grid_iq3s(uint32_t i) { return __ldg(&kGridIq3s[i]); }
 __device__ __forceinline__ uint64_t kk_grid_iq1s(uint32_t i) { return __ldg(&kGridIq1s[i]); }
 #define KK_DQ_DEV __device__ __forceinline__
-#include "kk_consume_core.cuh"
-#include "kk_dequant.cuh"
-
-// 2-D transpose tile (KK_OP_T_*): staged by the producer (t.bulk == 4) or, when a source row is not 16-byte aligned, gathered here.
-template <int ES, int CONV>
-__device__ __forceinline__ void run_t(const Dsts& D, const uint8_t* src, const TileDesc& t, uint32_t sbase, int ctid) {
-  const uint32_t nr = t.n_units & 0xFFFFu, nc = t.n_units >> 16;
-  uint32_t pitch = nc * ES;
-  if (t.bulk != 4) {
-    pitch = (pitch + 3u) & ~3u;
-    t_gather<ES>(src + t.src_off, sbase, pitch, nr, nc, t.C, ctid);
-    named_bar_consumers();
-  }
-  consume_t<ES, CONV>(D, sbase, pitch, nr, nc, t.R, t.col0, t.row0, t.dst_off, ctid);
-}
+#include "kk_consume_tile.cuh"
 
 __device__ __forceinline__ KKSeg load_seg(const KKSeg* p) {
   const uint4* q = reinterpret_cast<const uint4*>(p);
@@ -379,53 +369,7 @@ __global__ void __launch_bounds__(kThreads, 1) kk_convert_kernel(const ConvertLa
         mbar_arrive(empty0 + 8 * pending);
         pending = -1;
       }
-      // Block ops deal a tile's blocks (or groups of 4 / 8) to the 16 warps round-robin, and a full tile is rarely a multiple of 16 groups: a Q4_K tile
-      // is 56 quads — warps 0-7 would take 4 on EVERY tile, warps 8-15 three, and the pipeline runs at the pace of the busier half (0.875: exactly
-      // where Q4_K sat while Q5_K, whose 46.5 quads split almost evenly, reached 0.96 on the same code).  Rotating the warp numbering by half the
-      // warps on odd tiles gives every warp 4 + 3 over two tiles; outputs depend on the block, not on which warp expands it.
-      const int rwarp = (cwarp + (int)(it & 1u) * (kConsumerWarps / 2)) % kConsumerWarps;
-      switch (t.op) {
-        case KK_OP_ROWSPLIT: {  // unaligned fallback: byte-granular all-to-all copy
-          for (uint32_t k = ctid; k < t.n_units; k += kConsumerThreads) {
-            const KKRowSplitDst x = kk_rowsplit_byte(t, k);
-            L.xdst[x.j][x.off] = (uint8_t)lds8(pay + k);
-          }
-          break;
-        }
-        case KK_OP_COPY: consume_copy(D, pay, t.n_units, t.dst_off, ctid); break;
-        case KK_OP_F32_BF16: consume_f32(D, pay, t.n_units, t.dst_off, ctid); break;
-        case KK_OP_F16_BF16: consume_f16(D, pay, t.n_units, t.dst_off, ctid); break;
-        case KK_OP_Q4K_BF16: consume_q4k(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
-        case KK_OP_Q8_0_BF16: consume_q8_0(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
-        case KK_OP_Q6K_BF16: consume_q6k(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
-        case KK_OP_Q4_0_BF16: consume_legacy32<KK_Q4_0_BLOCK_BYTES, false, false>(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
-        case KK_OP_Q4_1_BF16: consume_legacy32<KK_Q4_1_BLOCK_BYTES, true, false>(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
-        case KK_OP_Q5_0_BF16: consume_legacy32<KK_Q5_0_BLOCK_BYTES, false, true>(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
-        case KK_OP_Q5_1_BF16: consume_legacy32<KK_Q5_1_BLOCK_BYTES, true, true>(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
-        case KK_OP_Q2K_BF16: consume_q2k(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
-        case KK_OP_Q3K_BF16: consume_q3k(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
-        case KK_OP_Q5K_BF16: consume_q5k(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
-        case KK_OP_IQ4NL_BF16: consume_codebook32<KK_IQ4NL_BLOCK_BYTES, 0>(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
-        case KK_OP_MXFP4_BF16: consume_codebook32<KK_MXFP4_BLOCK_BYTES, 1>(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
-        case KK_OP_IQ4XS_BF16: consume_iq4xs(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
-        case KK_OP_IQ2XXS_BF16: consume_iq2xxs(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
-        case KK_OP_IQ2XS_BF16: consume_iq2xs(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
-        case KK_OP_IQ2S_BF16: consume_iq2s(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
-        case KK_OP_IQ3XXS_BF16: consume_iq3xxs(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
-        case KK_OP_IQ3S_BF16: consume_iq3s(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
-        case KK_OP_IQ1S_BF16: consume_iq1s(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
-        case KK_OP_IQ1M_BF16: consume_iq1m(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
-        case KK_OP_TQ1_0_BF16: consume_tq1_0(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
-        case KK_OP_TQ2_0_BF16: consume_tq2_0(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
-        case KK_OP_NVFP4_BF16: consume_nvfp4(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
-        case KK_OP_F8E4M3_BF16: consume_f8<false>(D, pay, t.n_units, t.dst_off, ctid); break;
-        case KK_OP_F8E5M2_BF16: consume_f8<true>(D, pay, t.n_units, t.dst_off, ctid); break;
-        case KK_OP_T_F32_BF16: run_t<4, 1>(D, L.src, t, sbase, ctid); break;
-        case KK_OP_T_F16_BF16: run_t<2, 2>(D, L.src, t, sbase, ctid); break;
-        case KK_OP_T_B16: run_t<2, 0>(D, L.src, t, sbase, ctid); break;
-        case KK_OP_T_B32: run_t<4, 3>(D, L.src, t, sbase, ctid); break;
-        default: break;
-      }
+      kk_consume_tile(D, t, sbase, pay, L, cwarp, lane, ctid, it);
       __syncwarp();
       if (lane == 0) mbar_arrive(empty0 + 8 * s);
     }

@@ -1,13 +1,14 @@
-// Host emulation of kk_convert_kernel's block dequantisers.  TEST INFRASTRUCTURE ONLY.
+// Host emulation of kk_convert_kernel's consumer side.  TEST INFRASTRUCTURE ONLY.
 //
-// Compiles kukeon_b200/csrc/kk_dequant.cuh — the exact device source — with g++ by binding the handful of primitives it
-// uses (shared-memory loads, single-rounding fp32 arithmetic, bf16 packing, the 16-byte store) to plain C++, then plays
-// all 16 consumer warps x 32 lanes of one tile in a loop.  What this checks, on the CPU test tier, is the part of a
-// dequantiser that is easy to get wrong and cannot be seen by reading a formula: which lane reads which bytes of which
-// block and where its 16 output bytes land.  The bindings are stricter than the hardware: a misaligned 16/32-bit
-// shared load, a read outside the staged tile, a store outside the tile's output window or two stores to the same 16 bytes
-// all fail the run.  It does not check PTX spelling, memory ordering or anything about the producer warp; the -m gpu
-// parity tests do.  The product never links this file and has no CPU path.
+// Compiles kukeon_b200/csrc/kk_consume_tile.cuh — the kernel's per-tile dispatch and the consumer bodies it calls, the exact
+// device source — with g++ by binding the handful of primitives they use (shared-memory loads, single-rounding fp32
+// arithmetic, bf16 packing, the stores) to plain C++, then plays all 16 consumer warps x 32 lanes of a tile through
+// kk_consume_tile (play_tile).  What this checks, on the CPU test tier, is the part of a consumer that is easy to get wrong
+// and cannot be seen by reading a formula: which op runs which body with which arguments, which lane reads which bytes of
+// which block and where its output bytes land.  The bindings are stricter than the hardware: a misaligned 16/32-bit shared
+// load, a read outside the staged tile, a store outside the tile's output window or two stores to the same 16 bytes all fail
+// the run.  It does not check PTX spelling or memory ordering; the -m gpu parity tests do.  The product never links this file
+// and has no CPU path.
 #include <cmath>
 #include <cstdint>
 #include <algorithm>
@@ -18,6 +19,9 @@
 #include "../../kukeon_b200/csrc/kk_tile.h"
 
 namespace {
+
+constexpr int kConsumerWarps = KK_CONSUMER_WARPS;
+constexpr int kConsumerThreads = kConsumerWarps * 32;
 
 struct uint4 { uint32_t x, y, z, w; };
 struct uint2 { uint32_t x, y; };
@@ -36,13 +40,14 @@ struct Emu {
   uint8_t* hits = nullptr;  // one counter per 16 output bytes
   uint8_t* out_mask = nullptr;  // per 2 output bytes: written by a scalar (tail) store (per byte for store1_all: see byte_mask)
   uint8_t* byte_mask = nullptr; // per output byte: written by store1_all
-  // warp-shuffle emulation (see __shfl_sync below)
+  const uint8_t* src_end = nullptr;  // when set: kk_ldg8 must read below it (the end of the staged chunk)
+  // the pass of play_tile (1 record, 2 replay: see __shfl_sync below) and the thread it is playing
   static constexpr int kMaxShfl = 64;
-  int shfl_mode = 0, shfl_calls = 0, lane = 0;
-  float shfl_table[kMaxShfl][32];
+  int pass = 0, shfl_calls = 0, warp = 0, lane = 0;
   int err = 0;              // first failure: 1 load out of range, 2 misaligned load, 3 store out of range/misaligned, 4 double store
 };
 thread_local Emu g;
+thread_local float shfl_table[kConsumerWarps][Emu::kMaxShfl][32];  // per warp: the k-th shuffle / vote operand of every lane
 
 inline void flag(int e) { if (!g.err) g.err = e; }
 inline uint32_t lds8(uint32_t a) {
@@ -76,38 +81,27 @@ inline uint2 lds64(uint32_t a) {
   memcpy(&v, g.tile + a, 8);
   return v;
 }
-// Warp shuffle by record / replay: the driver runs every lane of a warp twice.  Pass 1 (g.shfl_mode == 1) records the value each lane
-// offers at its k-th shuffle and suppresses stores; pass 2 (== 2) hands out the recorded value of the source lane.  Valid for code whose
-// shuffled values do not depend on earlier shuffle results and whose lanes all execute the same shuffles (true of q4k_quad).
+// Warp shuffle by record / replay: play_tile runs every thread of a tile twice.  Pass 1 (g.pass == 1) records the value each lane offers
+// at its k-th shuffle and suppresses pool stores; pass 2 hands out the recorded value of the source lane of the same warp.  Valid for code
+// whose shuffled values do not depend on earlier shuffle results and whose lanes all execute the same shuffles (true of q4k_quad).
 inline float __shfl_sync(unsigned, float v, int src) {
-  if (g.shfl_mode == 1) {
-    if (g.shfl_calls >= Emu::kMaxShfl) { flag(7); return v; }
-    g.shfl_table[g.shfl_calls++][g.lane] = v;
-    return v;
-  }
-  if (g.shfl_mode == 2) {
-    if (g.shfl_calls >= Emu::kMaxShfl) { flag(7); return v; }
-    return g.shfl_table[g.shfl_calls++][src & 31];
-  }
-  flag(7);  // a shuffle outside record/replay cannot be emulated
-  return v;
+  if (g.shfl_calls >= Emu::kMaxShfl) { flag(7); return v; }
+  float* op = shfl_table[g.warp][g.shfl_calls++];
+  if (g.pass == 1) op[g.lane] = v;
+  return g.pass == 1 ? v : op[src & 31];
 }
 // Warp vote, by the same record / replay: pass 1 records every lane's predicate (and returns it: both arms of a vote-guarded branch must
 // issue the same shuffles, which they do — the vote only selects the arithmetic), pass 2 returns the AND over the 32 lanes.
 inline bool kk_all(bool p) {
-  if (g.shfl_mode == 1) {
-    if (g.shfl_calls >= Emu::kMaxShfl) { flag(7); return p; }
-    g.shfl_table[g.shfl_calls++][g.lane] = p ? 1.0f : 0.0f;
+  if (g.shfl_calls >= Emu::kMaxShfl) { flag(7); return p; }
+  float* op = shfl_table[g.warp][g.shfl_calls++];
+  if (g.pass == 1) {
+    op[g.lane] = p ? 1.0f : 0.0f;
     return p;
   }
-  if (g.shfl_mode == 2) {
-    if (g.shfl_calls >= Emu::kMaxShfl) { flag(7); return p; }
-    bool all = true;
-    for (int l = 0; l < 32; ++l) all = all && g.shfl_table[g.shfl_calls][l] != 0.0f;
-    g.shfl_calls++;
-    return all;
-  }
-  return p;
+  bool all = true;
+  for (int l = 0; l < 32; ++l) all = all && op[l] != 0.0f;
+  return all;
 }
 inline uint32_t kk_f2bits(float f) { uint32_t u; memcpy(&u, &f, 4); return u; }
 inline uint32_t kk_popc(uint32_t u) { return (uint32_t)__builtin_popcount(u); }
@@ -138,7 +132,10 @@ inline uint64_t kk_grid_iq2s(uint32_t i) { if (i >= KK_GRID_IQ2S_SIZE) { flag(8)
 inline uint32_t kk_grid_iq3xxs(uint32_t i) { if (i >= KK_GRID_IQ3XXS_SIZE) { flag(8); return 0; } return kGridIq3xxs[i]; }
 inline uint32_t kk_grid_iq3s(uint32_t i) { if (i >= KK_GRID_IQ3S_SIZE) { flag(8); return 0; } return kGridIq3s[i]; }
 inline uint64_t kk_grid_iq1s(uint32_t i) { if (i >= KK_GRID_IQ1S_SIZE) { flag(8); return 0; } return kGridIq1s[i]; }
-inline uint32_t kk_ldg8(const uint8_t* p) { return *p; }
+inline uint32_t kk_ldg8(const uint8_t* p) {
+  if (g.src_end && p >= g.src_end) { flag(11); return 0; }
+  return *p;
+}
 // PRMT (default mode) as the code under test uses it: selector nibble k (low 16 bits; the hardware ignores the rest) picks byte
 // (nibble & 7) of {b:a}.  Bit 3 of a nibble asks the hardware to replicate the byte's sign bit instead — never what this code wants, so a
 // selector that has it set is a failure (9), not something to mask away.
@@ -171,7 +168,7 @@ inline uint32_t pack_bf16x2(float a, float b) { return bf16_rne(a) | (bf16_rne(b
 struct Dsts { int unused; };
 // hits[u] counts the BYTES stored into 16-byte unit u: 16 after exactly one vector store (or eight 2-byte tail stores)
 inline void store16_all(const Dsts&, uint64_t off, const uint4& v) {
-  if (g.shfl_mode == 1) return;
+  if (g.pass == 1) return;
   if ((off & 15u) || off + 16 > g.out_bytes) { flag(3); return; }
   if (g.hits[off >> 4]) flag(4);
   g.hits[off >> 4] += 16;
@@ -180,7 +177,7 @@ inline void store16_all(const Dsts&, uint64_t off, const uint4& v) {
   for (int i = 0; i < g.n_more; ++i) memcpy(g.more_out[i] + off, &v, 16);
 }
 inline void store1_all(const Dsts&, uint64_t off, uint8_t v) {
-  if (g.shfl_mode == 1) return;
+  if (g.pass == 1) return;
   if (off + 1 > g.out_bytes) { flag(3); return; }
   if (g.byte_mask[off]) flag(4);
   g.byte_mask[off] = 1;
@@ -189,7 +186,7 @@ inline void store1_all(const Dsts&, uint64_t off, uint8_t v) {
   for (int i = 0; i < g.n_more; ++i) g.more_out[i][off] = v;
 }
 inline void store2_all(const Dsts&, uint64_t off, uint16_t v) {
-  if (g.shfl_mode == 1) return;
+  if (g.pass == 1) return;
   if ((off & 1u) || off + 2 > g.out_bytes) { flag(3); return; }
   if (g.out_mask[off >> 1]) flag(4);
   g.out_mask[off >> 1] = 1;
@@ -198,7 +195,7 @@ inline void store2_all(const Dsts&, uint64_t off, uint16_t v) {
   for (int i = 0; i < g.n_more; ++i) memcpy(g.more_out[i] + off, &v, 2);
 }
 inline void store8_all(const Dsts&, uint64_t off, uint32_t lo, uint32_t hi) {  // half an output vector: four entries of the 2-byte mask
-  if (g.shfl_mode == 1) return;
+  if (g.pass == 1) return;
   if ((off & 7u) || off + 8 > g.out_bytes) { flag(3); return; }
   for (int k = 0; k < 4; ++k) {
     if (g.out_mask[(off >> 1) + k]) flag(4);
@@ -210,7 +207,7 @@ inline void store8_all(const Dsts&, uint64_t off, uint32_t lo, uint32_t hi) {  /
   for (int i = 0; i < g.n_more; ++i) memcpy(g.more_out[i] + off, v, 8);
 }
 inline void store4_all(const Dsts&, uint64_t off, uint32_t v) {  // one 32-bit element (verbatim transposes): two entries of the 2-byte mask
-  if (g.shfl_mode == 1) return;
+  if (g.pass == 1) return;
   if ((off & 3u) || off + 4 > g.out_bytes) { flag(3); return; }
   if (g.out_mask[off >> 1] || g.out_mask[(off >> 1) + 1]) flag(4);
   g.out_mask[off >> 1] = g.out_mask[(off >> 1) + 1] = 1;
@@ -241,68 +238,64 @@ inline uint32_t f8_to_f16_bits(uint32_t b, bool e5m2) {
 template <bool E5M2>
 inline uint32_t kk_f8x2_to_f16x2(uint32_t v) { return f8_to_f16_bits(v, E5M2) | (f8_to_f16_bits(v >> 8, E5M2) << 16); }
 
-constexpr int kConsumerWarps = 16;  // must equal kConsumerWarps of kk_kernels.cu
-constexpr int kConsumerThreads = kConsumerWarps * 32;
+// The launch as kk_consume_tile sees it: the staged chunk (transposes gather from src) and, for KK_OP_ROWSPLIT, the pool of every rank
+// (ConvertLaunch::xdst) with its size, 16-byte hit counters and per-byte store mask.
+struct Launch {
+  const uint8_t* src = nullptr;
+  uint8_t* const* xdst = nullptr;
+  uint32_t n_xdst = 0;
+  const uint64_t* xpool_bytes = nullptr;
+  uint8_t* const* xhits = nullptr;
+  uint8_t* const* xmask1 = nullptr;
+};
+// A row-split store of `len` bytes into rank j's pool at `off`: the rank must have a pool, the bytes must lie inside it, and no byte of it may
+// have been stored before by any rank's launch.  Returns 0 or the failure code.
+int rowsplit_store(const Launch& L, uint32_t j, uint64_t off, const uint8_t* v, uint32_t len) {
+  if (j >= L.n_xdst || !L.xdst[j]) return 17;
+  if (off > L.xpool_bytes[j] || len > L.xpool_bytes[j] - off) return 15;
+  for (uint32_t i = 0; i < len; ++i) {
+    if (L.xmask1[j][off + i]) return 4;
+    L.xmask1[j][off + i] = 1;
+    L.xhits[j][(off + i) >> 4] += 1;
+  }
+  memcpy(L.xdst[j] + off, v, len);
+  return 0;
+}
+inline void rowsplit_store1(const Launch& L, uint32_t j, uint64_t off, uint8_t v) {
+  if (g.pass == 1) return;
+  if (int rc = rowsplit_store(L, j, off, &v, 1)) flag(rc);
+}
+// The consumer barrier: play_tile has every thread run its stage stores (pass 1) before any thread's consumer reads count (pass 2).
+inline void named_bar_consumers() {}
+
 #define KK_DQ_DEV static inline
 #define min(a, b) ((a) < (b) ? (a) : (b))
-#include "../../kukeon_b200/csrc/kk_consume_core.cuh"
-#include "../../kukeon_b200/csrc/kk_dequant.cuh"
+#include "../../kukeon_b200/csrc/kk_consume_tile.cuh"
 #undef min
 
-// (run_warps, below, plays all warps of a tile; ops that shuffle are run twice per warp)
-// One lane of the consumer side of a block / elementwise op — the same switch the kernel has.  false: op not covered here.
-inline bool run_op(uint32_t op, const Dsts& D, uint32_t pay, uint32_t n, uint64_t dst_off, int cwarp, int lane) {
-  switch (op) {
-    case KK_OP_Q8_0_BF16: consume_q8_0(D, pay, n, dst_off, cwarp, lane); return true;
-    case KK_OP_Q6K_BF16: consume_q6k(D, pay, n, dst_off, cwarp, lane); return true;
-    case KK_OP_Q4_0_BF16: consume_legacy32<KK_Q4_0_BLOCK_BYTES, false, false>(D, pay, n, dst_off, cwarp, lane); return true;
-    case KK_OP_Q4_1_BF16: consume_legacy32<KK_Q4_1_BLOCK_BYTES, true, false>(D, pay, n, dst_off, cwarp, lane); return true;
-    case KK_OP_Q5_0_BF16: consume_legacy32<KK_Q5_0_BLOCK_BYTES, false, true>(D, pay, n, dst_off, cwarp, lane); return true;
-    case KK_OP_Q5_1_BF16: consume_legacy32<KK_Q5_1_BLOCK_BYTES, true, true>(D, pay, n, dst_off, cwarp, lane); return true;
-    case KK_OP_Q2K_BF16: consume_q2k(D, pay, n, dst_off, cwarp, lane); return true;
-    case KK_OP_Q3K_BF16: consume_q3k(D, pay, n, dst_off, cwarp, lane); return true;
-    case KK_OP_Q5K_BF16: consume_q5k(D, pay, n, dst_off, cwarp, lane); return true;
-    case KK_OP_IQ4NL_BF16: consume_codebook32<KK_IQ4NL_BLOCK_BYTES, 0>(D, pay, n, dst_off, cwarp, lane); return true;
-    case KK_OP_MXFP4_BF16: consume_codebook32<KK_MXFP4_BLOCK_BYTES, 1>(D, pay, n, dst_off, cwarp, lane); return true;
-    case KK_OP_IQ4XS_BF16: consume_iq4xs(D, pay, n, dst_off, cwarp, lane); return true;
-    case KK_OP_IQ2XXS_BF16: consume_iq2xxs(D, pay, n, dst_off, cwarp, lane); return true;
-    case KK_OP_IQ2XS_BF16: consume_iq2xs(D, pay, n, dst_off, cwarp, lane); return true;
-    case KK_OP_IQ2S_BF16: consume_iq2s(D, pay, n, dst_off, cwarp, lane); return true;
-    case KK_OP_IQ3XXS_BF16: consume_iq3xxs(D, pay, n, dst_off, cwarp, lane); return true;
-    case KK_OP_IQ3S_BF16: consume_iq3s(D, pay, n, dst_off, cwarp, lane); return true;
-    case KK_OP_IQ1S_BF16: consume_iq1s(D, pay, n, dst_off, cwarp, lane); return true;
-    case KK_OP_IQ1M_BF16: consume_iq1m(D, pay, n, dst_off, cwarp, lane); return true;
-    case KK_OP_TQ1_0_BF16: consume_tq1_0(D, pay, n, dst_off, cwarp, lane); return true;
-    case KK_OP_TQ2_0_BF16: consume_tq2_0(D, pay, n, dst_off, cwarp, lane); return true;
-    case KK_OP_NVFP4_BF16: consume_nvfp4(D, pay, n, dst_off, cwarp, lane); return true;
-    case KK_OP_Q4K_BF16: consume_q4k(D, pay, n, dst_off, cwarp, lane); return true;
-    // elementwise ops: n = elements (COPY: bytes) of the tile, threads indexed 0..511 across the consumer warps
-    case KK_OP_COPY: consume_copy(D, pay, n, dst_off, cwarp * 32 + lane); return true;
-    case KK_OP_F32_BF16: consume_f32(D, pay, n, dst_off, cwarp * 32 + lane); return true;
-    case KK_OP_F16_BF16: consume_f16(D, pay, n, dst_off, cwarp * 32 + lane); return true;
-    case KK_OP_F8E4M3_BF16: consume_f8<false>(D, pay, n, dst_off, cwarp * 32 + lane); return true;
-    case KK_OP_F8E5M2_BF16: consume_f8<true>(D, pay, n, dst_off, cwarp * 32 + lane); return true;
-    default: return false;
-  }
+// One tile through kk_consume_tile, the kernel's dispatch, for all kConsumerWarps x 32 consumer threads, in two passes over all of them.
+// Pass 1 records every lane's shuffle and vote operands, per warp, and performs the stores into the stage, so a transpose's gather is
+// complete before pass 2 reads it; it suppresses pool stores.  Pass 2 replays the shuffles and votes, rewrites the same stage bytes and
+// stores.  it: the tile counter the kernel's warp rotation reads.  traces / straces (when given) receive each thread's pass-2 16/32-bit
+// shared loads and 16-byte store offsets.
+void play_tile(const KKTileDesc& t, const Launch& L, uint32_t it, std::vector<std::vector<uint32_t>>* traces = nullptr,
+               std::vector<std::vector<uint64_t>>* straces = nullptr) {
+  const Dsts D{0};
+  for (g.pass = 1; g.pass <= 2; ++g.pass)
+    for (int ctid = 0; ctid < kConsumerThreads; ++ctid) {
+      g.warp = ctid >> 5;
+      g.lane = ctid & 31;
+      g.shfl_calls = 0;
+      g.trace = g.pass == 2 && traces ? &(*traces)[(size_t)ctid] : nullptr;
+      g.strace = g.pass == 2 && straces ? &(*straces)[(size_t)ctid] : nullptr;
+      kk_consume_tile(D, t, 0, t.pay_off, L, g.warp, g.lane, ctid, it);
+    }
+  g.pass = 0;
+  g.trace = nullptr;
+  g.strace = nullptr;
 }
 
 }  // namespace
-
-inline bool run_warps(uint32_t op, const Dsts& D, uint32_t pay, uint32_t n, uint64_t dst_off) {
-  const bool shuffles = op == KK_OP_Q4K_BF16 || op == KK_OP_Q5K_BF16;
-  for (int cwarp = 0; cwarp < kConsumerWarps; ++cwarp) {
-    for (int pass = shuffles ? 1 : 0; pass <= (shuffles ? 2 : 0); ++pass) {
-      g.shfl_mode = pass;
-      for (int lane = 0; lane < 32; ++lane) {
-        g.lane = lane;
-        g.shfl_calls = 0;
-        if (!run_op(op, D, pay, n, dst_off, cwarp, lane)) return false;
-      }
-    }
-  }
-  g.shfl_mode = 0;
-  return true;
-}
 
 // Shared-memory wavefronts of per-lane load traces: the k-th recorded load of every lane of a warp is one warp instruction; it needs as
 // many wavefronts as the worst bank has distinct 4-byte words (same word = broadcast).  Adds to wavefronts / ideal.
@@ -330,52 +323,34 @@ void count_wavefronts(const std::vector<std::vector<uint32_t>>& traces, uint64_t
   }
 }
 
-// Run the consumer side of one tile of block op `op` (KKOp): `nblk` blocks whose first byte sits at tile[pay_off].
-// out receives nblk * out_bytes_per_block bytes; hits (out_bytes/16 counters, zeroed here) how often each 16-byte unit
-// was stored.  Returns 0, a positive Emu::err code, or -1 for an op this harness does not cover.
-extern "C" int kk_emul_dequant_tile(uint32_t op, const uint8_t* tile, uint32_t tile_bytes, uint32_t pay_off, uint32_t nblk, uint8_t* out,
-                                    uint64_t out_bytes, uint8_t* hits) {
+// Run the consumer side of one tile of block or elementwise op `op` (KKOp): `nblk` units whose first byte sits at tile[pay_off], additionally
+// reporting (when stats is given) the shared-memory wavefronts of the 16/32-bit loads (stats[0]) against one per warp load instruction
+// (stats[1]).  The wavefronts are only meaningful when all lanes of a warp execute the same loads (full warps of a full tile); byte loads
+// (lds8) and vector loads (lds64 / lds128) are not traced.  out receives nblk * out_bytes_per_block bytes; hits (out_bytes/16 counters,
+// zeroed here) how often each 16-byte unit was stored.  Returns 0, a positive Emu::err code, or -1 for a transpose or row-split op.
+extern "C" int kk_emul_dequant_tile_stats(uint32_t op, const uint8_t* tile, uint32_t tile_bytes, uint32_t pay_off, uint32_t nblk, uint8_t* out,
+                                          uint64_t out_bytes, uint8_t* hits, uint64_t* stats) {
+  if (kk_is_transpose(op) || op == KK_OP_ROWSPLIT) return -1;
   g = Emu{};
   g.tile = tile; g.tile_bytes = tile_bytes; g.out = out; g.out_bytes = out_bytes; g.hits = hits;
   memset(hits, 0, (out_bytes + 15) / 16);
   std::vector<uint8_t> mask(out_bytes / 2 + 1, 0), bmask(out_bytes + 1, 0);
   g.out_mask = mask.data();
   g.byte_mask = bmask.data();
-  const Dsts D{0};
-  if (!run_warps(op, D, pay_off, nblk, 0)) return -1;
+  KKTileDesc t{};
+  t.op = op; t.pay_off = pay_off; t.n_units = nblk;
+  std::vector<std::vector<uint32_t>> traces((size_t)kConsumerThreads);
+  play_tile(t, Launch{}, 0, stats ? &traces : nullptr);
+  if (stats) {
+    stats[0] = stats[1] = 0;
+    count_wavefronts(traces, stats[0], stats[1]);
+  }
   return g.err;
 }
 
-// Same as kk_emul_dequant_tile, additionally reporting the shared-memory wavefronts of the 16/32-bit loads (stats[0]) against one per warp
-// load instruction (stats[1]).  Only meaningful when all lanes of a warp execute the same loads (full warps of a full tile); byte loads
-// (lds8) and vector loads (lds64 / lds128) are not traced.  Ops that shuffle are traced in their replay pass.
-extern "C" int kk_emul_dequant_tile_stats(uint32_t op, const uint8_t* tile, uint32_t tile_bytes, uint32_t pay_off, uint32_t nblk, uint8_t* out,
-                                          uint64_t out_bytes, uint8_t* hits, uint64_t* stats) {
-  g = Emu{};
-  g.tile = tile; g.tile_bytes = tile_bytes; g.out = out; g.out_bytes = out_bytes; g.hits = hits;
-  memset(hits, 0, (out_bytes + 15) / 16);
-  std::vector<uint8_t> mask(out_bytes / 2 + 1, 0), bmask(out_bytes + 1, 0);
-  g.out_mask = mask.data();
-  g.byte_mask = bmask.data();
-  const Dsts D{0};
-  const bool shuffles = op == KK_OP_Q4K_BF16 || op == KK_OP_Q5K_BF16;
-  std::vector<std::vector<uint32_t>> traces((size_t)kConsumerWarps * 32);
-  for (int cwarp = 0; cwarp < kConsumerWarps; ++cwarp)
-    for (int pass = shuffles ? 1 : 0; pass <= (shuffles ? 2 : 0); ++pass) {
-      g.shfl_mode = pass;
-      for (int lane = 0; lane < 32; ++lane) {
-        g.lane = lane;
-        g.shfl_calls = 0;
-        g.trace = pass == 1 ? nullptr : &traces[(size_t)(cwarp * 32 + lane)];
-        if (!run_op(op, D, pay_off, nblk, 0, cwarp, lane)) return -1;
-      }
-    }
-  g.trace = nullptr;
-  g.shfl_mode = 0;
-  uint64_t wf = 0, ideal = 0;
-  count_wavefronts(traces, wf, ideal);
-  if (stats) { stats[0] = wf; stats[1] = ideal; }
-  return g.err;
+extern "C" int kk_emul_dequant_tile(uint32_t op, const uint8_t* tile, uint32_t tile_bytes, uint32_t pay_off, uint32_t nblk, uint8_t* out,
+                                    uint64_t out_bytes, uint8_t* hits) {
+  return kk_emul_dequant_tile_stats(op, tile, tile_bytes, pay_off, nblk, out, out_bytes, hits, nullptr);
 }
 
 // A whole segment the way the kernel walks it: the producer's per-tile arithmetic (kk_block_tile, the same function the
@@ -406,8 +381,9 @@ extern "C" int kk_emul_dequant_segment(uint32_t op, const uint8_t* src, uint64_t
     g.tile = stage; g.tile_bytes = mis + bt.in_bytes; g.out = out; g.out_bytes = out_bytes; g.hits = hits;
     g.out_mask = mask.data();
     g.byte_mask = bmask.data();
-    const Dsts D{0};
-    if (!run_warps(op, D, mis, bt.n_blocks, bt.dst_off)) return -1;
+    KKTileDesc d{};
+    d.op = op; d.pay_off = mis; d.n_units = bt.n_blocks; d.dst_off = bt.dst_off;
+    play_tile(d, Launch{}, (uint32_t)t);
     if (g.err) return g.err;
   }
   return 0;
@@ -427,60 +403,24 @@ extern "C" int kk_emul_t_tile(uint32_t op, const uint8_t* src, uint32_t C, uint3
   if (nr > KK_T_ROWS || nc * es > KK_T_ROW_BYTES) return 5;
   static thread_local uint8_t stage[KK_TILE_SRC_BYTES + KK_STAGE_PAD];
   memset(stage, 0xEE, sizeof stage);
-  uint32_t pitch = nc * es;
   std::vector<uint8_t> mask(dst_bytes / 2 + 1, 0), bmask(dst_bytes + 1, 0);
   memset(hits, 0, (dst_bytes + 15) / 16);
   g = Emu{};
   g.tile = stage; g.wtile = stage; g.tile_bytes = sizeof stage; g.out = dst; g.out_bytes = dst_bytes; g.hits = hits; g.out_mask = mask.data();
   g.byte_mask = bmask.data();
-  const Dsts D{0};
-  const int nthreads = kConsumerWarps * 32;
-  if (staged) {
-    for (uint32_t r = 0; r < nr; ++r) memcpy(stage + r * pitch, src + (uint64_t)r * C * es, (size_t)nc * es);
-  } else {
-    pitch = (pitch + 3u) & ~3u;
-    for (int t = 0; t < nthreads; ++t) {
-      if (es == 4) t_gather<4>(src, 0, pitch, nr, nc, C, t);
-      else t_gather<2>(src, 0, pitch, nr, nc, C, t);
-    }
-    // (the kernel has a named barrier here)
-  }
-  std::vector<std::vector<uint32_t>> traces((size_t)nthreads);
-  std::vector<std::vector<uint64_t>> straces((size_t)nthreads);
-  for (int t = 0; t < nthreads; ++t) {
-    g.trace = &traces[(size_t)t];
-    g.strace = &straces[(size_t)t];
-    switch (op) {
-      case KK_OP_T_F32_BF16: consume_t<4, 1>(D, 0, pitch, nr, nc, R, col0, row0, 0, t); break;
-      case KK_OP_T_F16_BF16: consume_t<2, 2>(D, 0, pitch, nr, nc, R, col0, row0, 0, t); break;
-      case KK_OP_T_B16: consume_t<2, 0>(D, 0, pitch, nr, nc, R, col0, row0, 0, t); break;
-      default: consume_t<4, 3>(D, 0, pitch, nr, nc, R, col0, row0, 0, t); break;
-    }
-  }
-  g.trace = nullptr;
-  g.strace = nullptr;
+  KKTileDesc t{};
+  t.op = op; t.n_units = nr | (nc << 16); t.bulk = staged ? 4 : 0; t.C = C; t.R = R; t.col0 = col0; t.row0 = row0;
+  if (staged)
+    for (uint32_t r = 0; r < nr; ++r) memcpy(stage + r * nc * es, src + (uint64_t)r * C * es, (size_t)nc * es);
+  Launch L;
+  L.src = src;
+  std::vector<std::vector<uint32_t>> traces((size_t)kConsumerThreads);
+  std::vector<std::vector<uint64_t>> straces((size_t)kConsumerThreads);
+  play_tile(t, L, 0, &traces, &straces);
   uint64_t wavefronts = 0, ideal = 0, st_instr = 0, st_lines = 0, st_sectors = 0;
+  count_wavefronts(traces, wavefronts, ideal);
   for (int w = 0; w < kConsumerWarps; ++w) {
     size_t longest = 0;
-    for (int l = 0; l < 32; ++l) longest = std::max(longest, traces[(size_t)(32 * w + l)].size());
-    for (size_t k = 0; k < longest; ++k) {  // the k-th shared load of every lane of the warp is one warp instruction
-      std::vector<uint32_t> words[32];
-      bool any = false;
-      for (int l = 0; l < 32; ++l) {
-        const auto& tr = traces[(size_t)(32 * w + l)];
-        if (k >= tr.size()) continue;
-        any = true;
-        const uint32_t word = tr[k] >> 2;
-        auto& v = words[word & 31u];
-        if (std::find(v.begin(), v.end(), word) == v.end()) v.push_back(word);
-      }
-      if (!any) continue;
-      size_t worst = 1;
-      for (auto& v : words) worst = std::max(worst, v.size());
-      wavefronts += worst;
-      ideal += 1;
-    }
-    longest = 0;
     for (int l = 0; l < 32; ++l) longest = std::max(longest, straces[(size_t)(32 * w + l)].size());
     for (size_t k = 0; k < longest; ++k) {  // likewise the k-th 16-byte store
       std::vector<uint64_t> lines, sectors;
@@ -501,26 +441,10 @@ extern "C" int kk_emul_t_tile(uint32_t op, const uint8_t* src, uint32_t C, uint3
   return g.err;
 }
 
-// A row-split store of `len` bytes into rank j's pool at `off`: the rank must have a pool, the bytes must lie inside it, and no byte of it may
-// have been stored before by any rank's launch.  Returns 0 or the failure code.
-static int rowsplit_store(uint8_t* const* xdst, uint32_t n_xdst, const uint64_t* xpool_bytes, uint8_t* const* xhits, uint8_t* const* xmask1,
-                          uint32_t j, uint64_t off, const uint8_t* v, uint32_t len) {
-  if (j >= n_xdst || !xdst[j]) return 17;
-  if (off > xpool_bytes[j] || len > xpool_bytes[j] - off) return 15;
-  for (uint32_t i = 0; i < len; ++i) {
-    if (xmask1[j][off + i]) return 4;
-    xmask1[j][off + i] = 1;
-    xhits[j][(off + i) >> 4] += 1;
-  }
-  memcpy(xdst[j] + off, v, len);
-  return 0;
-}
-
 // A whole launch of kk_convert_kernel, tile by tile: resolve the tile's segment from tile_begin[] (as the producer does), kk_make_tile (the
 // function the kernel's producer calls), perform the bulk copies it asks for into a stage buffer with the hardware's constraints checked
-// (16-byte aligned source, destination and size; bytes issued == bytes announced), then the consumer side: the aligned-copy bulk stores, the
-// row-split exchange through the kernel's own addressing (kk_rowsplit_*), or the same per-lane device functions the other entry points run,
-// for all 16 x 32 consumer lanes.
+// (16-byte aligned source, destination and size; bytes issued == bytes announced), then the consumer side: the kernel's two bulk-store paths
+// (aligned copy, aligned row-split exchange), or every other tile through kk_consume_tile (play_tile) with the launch's tile counter.
 // src: the staged chunk (src base assumed 256-byte aligned like the staging buffers); dst[0..n_dst): destination pools of pool_bytes each;
 // hits / masks describe dst[0] and ACCUMULATE across calls (the caller zeroes them once per pool).
 // xdst[0..n_xdst): the pool of every rank, for KK_OP_ROWSPLIT tiles (ConvertLaunch::xdst); xpool_bytes, xhits and xmask1 are each pool's
@@ -531,6 +455,8 @@ extern "C" int kk_emul_launch(const uint8_t* src, uint64_t src_bytes, const KKSe
                               uint8_t* const* xdst, uint32_t n_xdst, const uint64_t* xpool_bytes, uint8_t* const* xhits, uint8_t* const* xmask1,
                               uint64_t* rs_tiles) {
   if (n_dst < 1 || n_dst > KK_MAX_DST) return -1;
+  Launch L;
+  L.src = src; L.xdst = xdst; L.n_xdst = n_xdst; L.xpool_bytes = xpool_bytes; L.xhits = xhits; L.xmask1 = xmask1;
   static thread_local uint8_t stage[KK_TILE_SRC_BYTES + KK_STAGE_PAD];
   const uint64_t src_addr = 0x100000;  // only the alignment of the src base matters
   uint32_t cur = 0;
@@ -569,8 +495,7 @@ extern "C" int kk_emul_launch(const uint8_t* src, uint64_t src_bytes, const KKSe
     g.out = dst[0]; g.out_bytes = pool_bytes; g.hits = hits; g.out_mask = mask2; g.byte_mask = mask1;
     g.n_more = (int)n_dst - 1;
     for (int i = 0; i < g.n_more; ++i) g.more_out[i] = dst[i + 1];
-    const Dsts D{0};
-    const uint32_t nr = d.n_units & 0xFFFFu, nc = d.n_units >> 16;
+    g.src_end = src + src_bytes;
     if (d.bulk == 1) {  // aligned verbatim copy: one bulk store from the stage to every pool
       if ((d.dst_off & 15u) || (d.n_units & 15u) || (d.pay_off & 15u) || d.dst_off + d.n_units > pool_bytes) return 13;
       for (uint32_t u = 0; u < d.n_units; u += 16) {
@@ -580,56 +505,22 @@ extern "C" int kk_emul_launch(const uint8_t* src, uint64_t src_bytes, const KKSe
       for (uint32_t i = 0; i < n_dst; ++i) memcpy(dst[i] + d.dst_off, stage + d.pay_off, d.n_units);
       continue;
     }
-    if (d.op == KK_OP_ROWSPLIT) {
-      if (!d.C || !d.R) return 18;  // the kernel would divide by zero
-      if (d.bulk == 3) {  // one bulk store per (row, rank) piece, from warp 0 lane 0
-        for (KKRowSplitWalk w = kk_rowsplit_walk(d); w.pos < w.end;) {
-          const KKRowSplitPiece p = kk_rowsplit_piece(d, w);
-          const uint32_t s0 = d.pay_off + p.src;
-          if ((p.dst.off & 15u) || (s0 & 15u) || (p.len & 15u) || !p.len) return 14;
-          if (s0 + p.len > staged) return 16;
-          if (int rc = rowsplit_store(xdst, n_xdst, xpool_bytes, xhits, xmask1, p.dst.j, p.dst.off, stage + s0, p.len)) return rc;
-          kk_rowsplit_advance(d, w, p.len);
-        }
-      } else {  // byte-granular consumer: every consumer thread strides over the tile
-        for (int t = 0; t < kConsumerThreads; ++t)
-          for (uint32_t k = (uint32_t)t; k < d.n_units; k += kConsumerThreads) {
-            const KKRowSplitDst x = kk_rowsplit_byte(d, k);
-            if (d.pay_off + k >= staged) return 16;
-            if (int rc = rowsplit_store(xdst, n_xdst, xpool_bytes, xhits, xmask1, x.j, x.off, stage + d.pay_off + k, 1)) return rc;
-          }
+    if (d.op == KK_OP_ROWSPLIT && (!d.C || !d.R)) return 18;  // the kernel would divide by zero
+    if (d.bulk == 3) {  // row-split exchange, aligned: one bulk store per (row, rank) piece, from warp 0 lane 0
+      for (KKRowSplitWalk w = kk_rowsplit_walk(d); w.pos < w.end;) {
+        const KKRowSplitPiece p = kk_rowsplit_piece(d, w);
+        const uint32_t s0 = d.pay_off + p.src;
+        if ((p.dst.off & 15u) || (s0 & 15u) || (p.len & 15u) || !p.len) return 14;
+        if (s0 + p.len > staged) return 16;
+        if (int rc = rowsplit_store(L, p.dst.j, p.dst.off, stage + s0, p.len)) return rc;
+        kk_rowsplit_advance(d, w, p.len);
       }
-      if (rs_tiles) ++rs_tiles[d.bulk == 3 ? 0 : 1];
+      if (rs_tiles) ++rs_tiles[0];
       continue;
     }
-    switch (d.op) {
-      case KK_OP_T_F32_BF16: case KK_OP_T_F16_BF16: case KK_OP_T_B16: case KK_OP_T_B32: {
-        const uint32_t es = kk_t_src_es(d.op);
-        uint32_t pitch = nc * es;
-        if (d.bulk != 4u) {  // run_t of the kernel: gather, (barrier), consume
-          pitch = (pitch + 3u) & ~3u;
-          g.tile_bytes = (uint32_t)sizeof stage;
-          if (d.src_off + ((uint64_t)(nr ? nr - 1 : 0) * d.C + nc) * es > src_bytes) return 11;
-          for (int t = 0; t < kConsumerThreads; ++t) {
-            if (es == 4) t_gather<4>(src + d.src_off, 0, pitch, nr, nc, d.C, t);
-            else t_gather<2>(src + d.src_off, 0, pitch, nr, nc, d.C, t);
-          }
-        }
-        for (int t = 0; t < kConsumerThreads; ++t) {
-          switch (d.op) {
-            case KK_OP_T_F32_BF16: consume_t<4, 1>(D, 0, pitch, nr, nc, d.R, d.col0, d.row0, d.dst_off, t); break;
-            case KK_OP_T_F16_BF16: consume_t<2, 2>(D, 0, pitch, nr, nc, d.R, d.col0, d.row0, d.dst_off, t); break;
-            case KK_OP_T_B16: consume_t<2, 0>(D, 0, pitch, nr, nc, d.R, d.col0, d.row0, d.dst_off, t); break;
-            default: consume_t<4, 3>(D, 0, pitch, nr, nc, d.R, d.col0, d.row0, d.dst_off, t); break;
-          }
-        }
-        break;
-      }
-      default:
-        if (!run_warps(d.op, D, d.pay_off, d.n_units, d.dst_off)) return -1;
-        break;
-    }
+    play_tile(d, L, tile);
     if (g.err) return g.err;
+    if (d.op == KK_OP_ROWSPLIT && rs_tiles) ++rs_tiles[1];
   }
   return 0;
 }

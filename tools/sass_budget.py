@@ -1,7 +1,7 @@
 """Static instruction budget of kk_convert_kernel's consumer loops, read from the SASS (no GPU needed).
 
-For every `case KK_OP_*:` of the consumer dispatch in csrc/kk_kernels.cu this attributes the kernel's SASS instructions to the op whose
-dispatch line they were inlined at (`nvdisasm -gi`, built with -lineinfo), finds the op's loops from the backward branches, and reports for
+For every `case KK_OP_*:` of the consumer dispatch (kk_consume_tile in csrc/kk_consume_tile.cuh) this attributes the kernel's SASS
+instructions to the op whose dispatch line they were inlined at (`nvdisasm -gi`, built with -lineinfo), finds the op's loops from the backward branches, and reports for
 the op's main loop: warp instructions per iteration, the opcode mix, and — with the bytes one warp iteration reads and writes — warp
 instructions per KiB of algorithmic HBM traffic.  Put against the issue rate of the machine (4 schedulers x 1 warp instruction per clock per
 SM) this gives the traffic rate at which the loop would saturate instruction issue: a loop whose ceiling is below the HBM roofline is
@@ -23,6 +23,7 @@ import tempfile
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "kukeon_b200", "csrc")
 KERNEL_CU = os.path.join(CSRC, "kk_kernels.cu")
+DISPATCH = os.path.join(CSRC, "kk_consume_tile.cuh")
 
 SM_COUNT, SM_GHZ, ISSUE_PER_CLK = 132, 1.98, 4  # H100 SXM: 132 SMs, 1980 MHz sampled during bench.py's timed steps (700 W limit), 4 warp schedulers per SM
 HBM_PEAK_GBS = 3350.0                           # H100 SXM data sheet (HBM3); the store-only probe measured 3,165 GB/s on the same card
@@ -75,7 +76,8 @@ def disassemble(obj=None):
 
 
 def parse(text):
-    """-> list of dicts for the instructions of kk_convert_kernel: idx, op (mnemonic), outer (line of kk_kernels.cu the chain ends at), label index map."""
+    """-> list of dicts for the instructions of kk_convert_kernel: idx, op (mnemonic), chain (the inline frames (file, line, inlined-at file,
+    inlined-at line), innermost first), label index map."""
     lines = text.split("\n")
     start = next(i for i, l in enumerate(lines) if l.startswith(".text.") and "kk_convert_kernel" in l)
     ins, labels = [], {}
@@ -99,22 +101,26 @@ def parse(text):
         m = re.match(r"/\*([0-9a-f]+)\*/\s+(@!?U?P\d+\s+)?([A-Z0-9_.]+)\s*(.*);", s)
         if m:
             fresh = True
-            outer = None
-            if chain:
-                f, ln, f2, ln2 = chain[-1]
-                outer = (f2, ln2) if f2 else (f, ln)
-            ins.append({"i": len(ins), "pred": (m.group(2) or "").strip(), "mn": m.group(3), "args": m.group(4), "outer": outer,
-                        "inner": chain[0][:2] if chain else None})
+            ins.append({"i": len(ins), "pred": (m.group(2) or "").strip(), "mn": m.group(3), "args": m.group(4), "chain": chain})
     return ins, labels
 
 
 def dispatch_lines():
     out = {}
-    for n, l in enumerate(open(KERNEL_CU), 1):
+    for n, l in enumerate(open(DISPATCH), 1):
         m = re.match(r"\s*case (KK_OP_\w+):", l)
         if m:
             out[n] = m.group(1)
     return out
+
+
+def dispatch_op(chain, disp):
+    """The op whose `case` line the instruction was inlined at: the frame inlined at a dispatch line, or code on that line itself."""
+    for f, ln, f2, ln2 in reversed(chain):
+        for ff, ll in ((f2, ln2), (f, ln)):
+            if ff and ff.endswith(os.path.basename(DISPATCH)) and ll in disp:
+                return disp[ll]
+    return None
 
 
 def loops_of(ins, labels):
@@ -190,10 +196,7 @@ def classify(mn):
 def analyse():
     ins, labels = parse(disassemble())
     disp = dispatch_lines()
-    owner = []
-    for x in ins:
-        o = x["outer"]
-        owner.append(disp.get(o[1]) if o and o[0].endswith("kk_kernels.cu") else None)
+    owner = [dispatch_op(x["chain"], disp) for x in ins]
     loops = loops_of(ins, labels)
     rows = []
     for op in dict.fromkeys(disp.values()):
