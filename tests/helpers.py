@@ -1,6 +1,8 @@
-"""Test helpers: small checkpoint builders and a CPU emulator of kk_plan_describe output."""
+"""Test helpers: small checkpoint builders, a CPU emulator of kk_plan_describe output, and the poison-and-check pair that the GPU tests
+compare whole pools with (poison, assert_pool_exact)."""
 from __future__ import annotations
 
+import itertools
 import json
 import os
 import struct
@@ -164,6 +166,91 @@ def expected_mask(plan_pool: List[dict], total: int) -> np.ndarray:
     for p in plan_pool:
         m[p["pool_offset"]:p["pool_offset"] + p["nbytes"]] = True
     return m
+
+
+_POISON_SEEDS = itertools.count(1)
+
+
+def poison(m, device: int, seed: int | None = None) -> np.ndarray:
+    """Overwrite `device`'s whole pool of model `m`, [pool_ptr, pool_ptr + pool_bytes) and nothing else, with Philox-random bytes
+    (a fresh seed per call unless one is given) and return them: whatever a later launch does not write still holds these bytes, so
+    assert_pool_exact can tell a skipped store from a correct one even when the pool's memory held the answer before."""
+    from cuda.bindings import runtime as cudart
+    ptr, n = m.pool_ptr(device)
+    s = next(_POISON_SEEDS) if seed is None else seed
+    fill = np.frombuffer(np.random.Generator(np.random.Philox(s)).bytes(n), np.uint8).copy()
+    err, = cudart.cudaMemcpy(ptr, fill.ctypes.data, n, cudart.cudaMemcpyKind.cudaMemcpyHostToDevice)
+    assert err == cudart.cudaError_t.cudaSuccess, err
+    err, = cudart.cudaDeviceSynchronize()  # a pageable H2D copy may return before its DMA has landed
+    assert err == cudart.cudaError_t.cudaSuccess, err
+    return fill
+
+
+class PoolMismatch(AssertionError):
+    """assert_pool_exact's failure; `.findings` lists (class, region, first offset, byte count) per region and class, where class is
+    "unwritten" (inside the expected footprint, still the poison), "wrong value" (inside it, neither poison nor the expected byte) or
+    "stray store" (outside it, no longer the poison)."""
+
+    def __init__(self, label: str, findings: List[Tuple[str, str, int, int]]):
+        self.findings = findings
+        lines = [f"{c}: {n} B in {where}, first at pool offset {off}" for c, where, off, n in findings[:12]]
+        more = f"\n  ... {len(findings) - 12} more" if len(findings) > 12 else ""
+        super().__init__(f"{label}: pool differs\n  " + "\n  ".join(lines) + more)
+
+
+def _regions(placements: Sequence[Tuple[str, int, int]], total: int) -> Tuple[np.ndarray, List[str]]:
+    """Cut [0, total) into named placements and the gaps between them: (start offsets, names)."""
+    starts, names, at, prev = [], [], 0, None
+    for name, a, nb in sorted((p for p in placements if p[2] > 0), key=lambda p: p[1]):
+        if a > at:
+            starts.append(at)
+            names.append(f"gap between {prev} and {name}" if prev else f"gap before {name}")
+        starts.append(a)
+        names.append(name)
+        at, prev = a + nb, name
+    if at < total or not starts:
+        starts.append(at)
+        names.append(f"tail after {prev}" if prev else "pool")
+    return np.array(starts, np.int64), names
+
+
+def check_pool_bytes(got: np.ndarray, exp: np.ndarray, mask: np.ndarray, fill: np.ndarray, placements: Sequence[Tuple[str, int, int]],
+                     label: str, may_rewrite: np.ndarray | None = None) -> None:
+    """The whole pool `got` against `exp` where `mask` is set and against the poison `fill` everywhere else; raises PoolMismatch.
+    placements: (name, pool offset, nbytes) to name where a difference lies; may_rewrite: bytes outside `mask` a load is allowed to
+    change (PULL's gap bytes, see test_pull_fan_out_virtual_ranks_on_one_gpu)."""
+    assert got.shape == exp.shape == mask.shape == fill.shape, (got.shape, exp.shape, mask.shape, fill.shape)
+    diff = got != exp
+    classes = [("unwritten", mask & diff & (got == fill)), ("wrong value", mask & diff & (got != fill))]
+    stray = ~mask & (got != fill)
+    if may_rewrite is not None:
+        stray &= ~may_rewrite
+    classes.append(("stray store", stray))
+    if not any(c.any() for _, c in classes):
+        return
+    starts, names = _regions(placements, len(got))
+    findings = []
+    for cls, sel in classes:
+        idx = np.flatnonzero(sel)
+        if not idx.size:
+            continue
+        reg = np.searchsorted(starts, idx, side="right") - 1
+        cut = np.flatnonzero(np.diff(reg)) + 1
+        for grp in np.split(np.arange(idx.size), cut):
+            findings.append((cls, names[max(int(reg[grp[0]]), 0)], int(idx[grp[0]]), int(grp.size)))
+    findings.sort(key=lambda f: f[2])
+    raise PoolMismatch(label, findings)
+
+
+def assert_pool_exact(m, device: int, exp: np.ndarray, mask: np.ndarray, fill: np.ndarray, label: str,
+                      may_rewrite: np.ndarray | None = None) -> None:
+    """Read `device`'s whole pool and check every byte (check_pool_bytes); differences are named by the model's own placements."""
+    _, n = m.pool_ptr(device)
+    assert n == len(exp), f"{label}: the pool holds {n} B, the oracle's layout {len(exp)} B"
+    pls = []
+    for t in m.tensors():
+        pls += [(t["name"], p.pool_offset, p.nbytes) for p in m.placements(t["name"]) if p.device == device]
+    check_pool_bytes(m.read(device, 0, n), exp, mask, fill, pls, label, may_rewrite)
 
 
 def write_raw_safetensors(path: str, header: dict | bytes, data: bytes, n_override: int | None = None) -> None:

@@ -29,7 +29,20 @@ def assert_pool_matches(m, device, shards, recs, mode=0, flags=0, n_parts=1, par
     return exp, plan
 
 
+def expected_exact(shards, recs, mode=0, flags=0, n_parts=1, part=0):
+    """(whole expected pool, its written-byte mask) of one device: every placement's bytes, nothing in the gaps or the tail."""
+    exp, plan = oracle.expected_pool(shards, recs, mode, flags, n_parts, part)
+    return exp, helpers.expected_mask(plan, len(exp))
+
+
+def poison_all(ms, device=0):
+    return [helpers.poison(m, device) for m in ms]
+
+
 def load_and_check(pool, path, **kw):
+    """A plain load checked placement by placement, then the same file again over poisoned pools: a deferred load, the streaming
+    conversion and three resident conversions (the last two back to back, each starting from the scheduler counters the previous
+    launch left), every one checked byte for byte over the whole pool."""
     shards, recs = oracle.index_path(path)
     m = pool.load(path, **kw)
     try:
@@ -37,7 +50,31 @@ def load_and_check(pool, path, **kw):
         exp, plan = assert_pool_matches(m, pool.devices[0], shards, recs, flags=kw.get("flags", 0))
         for p in plan[:4]:
             assert m.checksum(pool.devices[0], p["pool_offset"], p["nbytes"]) == oracle.checksum(exp[p["pool_offset"]:p["pool_offset"] + p["nbytes"]])
-        return m.stats()
+        st = m.stats()
+    finally:
+        m.release()
+    poisoned_load_and_convert(pool, path, shards, recs, **kw)
+    return st
+
+
+def poisoned_load_and_convert(pool, path, shards, recs, mode=gpupool.MODE_SINGLE, fanout=gpupool.FANOUT_P2P, flags=0):
+    dev = pool.devices[0]
+    exp, mask = expected_exact(shards, recs, flags=flags)  # one device: BROADCAST lays the pool out as SINGLE does
+    raw = fanout == gpupool.FANOUT_RAW  # RAW converts in a second stage, from the raw image
+    m = pool.load(path, mode=mode, fanout=fanout, flags=flags | gpupool.LOAD_DEFER)
+    try:
+        fill = helpers.poison(m, dev)
+        m.load_part()
+        if raw:
+            m.convert_local()
+        helpers.assert_pool_exact(m, dev, exp, mask, fill, f"{os.path.basename(path)}: streaming load")
+        m.stage_resident()
+        for k in range(3):
+            fill = helpers.poison(m, dev)
+            m.convert_resident()
+            if raw:
+                m.convert_local()
+            helpers.assert_pool_exact(m, dev, exp, mask, fill, f"{os.path.basename(path)}: resident conversion {k + 1}")
     finally:
         m.release()
 
@@ -327,16 +364,19 @@ def test_resident_convert_equals_streaming_load(native, tmp_path):
         m = pl.load(d, flags=gpupool.LOAD_DEFER)
         try:
             assert not m.info()["loaded"]
+            exp, mask = expected_exact(shards, recs)
+            fill = helpers.poison(m, 0)
             m.stage_resident()
             tot, per = m.convert_resident()
             assert tot > 0 and len(per) == len(shards), "one launch per shard"
-            assert_pool_matches(m, 0, shards, recs)
+            helpers.assert_pool_exact(m, 0, exp, mask, fill, "resident conversion")
             m.unstage_resident()
+            fill = helpers.poison(m, 0)
             with pytest.raises(gpupool.ErrState):
                 m.convert_resident()
             m.load_part()
             assert m.info()["loaded"]
-            assert_pool_matches(m, 0, shards, recs)
+            helpers.assert_pool_exact(m, 0, exp, mask, fill, "streaming load after the resident image was dropped")
         finally:
             m.release()
 
@@ -488,24 +528,25 @@ sys.path.insert(0, sys.argv[1])
 import numpy as np
 from kukeon_b200 import gpupool
 from oracle import oracle
+from tests import helpers
 paths = sys.argv[2:]
+nd = os.environ['KUKEON_GPULOAD_TEST_NDST']
 with gpupool.Pool([0], n_staging_buffers=2, staging_buffer_bytes=1 << 20, n_reader_threads=1) as pl:
     for spec in paths:
         path, flags = spec.rsplit(":", 1)
         flags = int(flags)
         shards, recs = oracle.index_path(path)
-        m = pl.load(path, flags=flags)
+        m = pl.load(path, flags=flags | gpupool.LOAD_DEFER)
         try:
             exp, plan = oracle.expected_pool(shards, recs, 0, flags)
-            got = m.read(0, 0, len(exp))
-            for p in plan:
-                a, b = p["pool_offset"], p["pool_offset"] + p["nbytes"]
-                assert np.array_equal(got[a:b], exp[a:b]), f"n_dst={os.environ['KUKEON_GPULOAD_TEST_NDST']}: {p['name']} differs"
-            m.stage_resident(); m.convert_resident()
-            got = m.read(0, 0, len(exp))
-            for p in plan:
-                a, b = p["pool_offset"], p["pool_offset"] + p["nbytes"]
-                assert np.array_equal(got[a:b], exp[a:b]), f"resident n_dst={os.environ['KUKEON_GPULOAD_TEST_NDST']}: {p['name']} differs"
+            mask = helpers.expected_mask(plan, len(exp))
+            fill = helpers.poison(m, 0)
+            m.load_part()
+            helpers.assert_pool_exact(m, 0, exp, mask, fill, f"n_dst={nd} {spec}")
+            m.stage_resident()
+            fill = helpers.poison(m, 0)
+            m.convert_resident()
+            helpers.assert_pool_exact(m, 0, exp, mask, fill, f"resident n_dst={nd} {spec}")
         finally:
             m.release()
 print("ok")
@@ -550,13 +591,16 @@ def test_raw_fanout_degenerates_on_one_gpu(pool, tmp_path):
     shards, recs = oracle.index_path(g)
     m = pool.load(g, mode=gpupool.MODE_BROADCAST, fanout=gpupool.FANOUT_RAW, flags=gpupool.LOAD_DEFER)
     try:
+        exp, mask = expected_exact(shards, recs)
+        fill = helpers.poison(m, 0)
         m.load_part()
         m.convert_local()
-        assert_pool_matches(m, 0, shards, recs)
+        helpers.assert_pool_exact(m, 0, exp, mask, fill, "RAW stage 2")
         m.stage_resident()
+        fill = helpers.poison(m, 0)
         tot, per = m.convert_resident()  # no peers: nothing to fan out
         assert per == [] and m.convert_local() > 0
-        assert_pool_matches(m, 0, shards, recs)
+        helpers.assert_pool_exact(m, 0, exp, mask, fill, "RAW stage 2 from the resident image")
     finally:
         m.release()
 
@@ -587,17 +631,20 @@ def test_virtual_ranks_broadcast_on_one_gpu(pool, tmp_path, n):
     for path, flags in ((d, 0), (g, 0), (f, gpupool.LOAD_GPT2_CONV1D_T)):
         shards, recs = oracle.index_path(path)
         ms = _virtual_ranks(pool, path, gpupool.MODE_BROADCAST, n, flags)
+        exp, mask = expected_exact(shards, recs, flags=flags)
         try:
+            fills = poison_all(ms)
             for m in ms:
                 m.load_part()  # rank i converts its 1/n and stores it into all n pools
-            for m in ms:
-                assert_pool_matches(m, 0, shards, recs, flags=flags)
+            for i, (m, fill) in enumerate(zip(ms, fills)):
+                helpers.assert_pool_exact(m, 0, exp, mask, fill, f"{os.path.basename(path)} rank {i} of {n}")
             for m in ms:       # and again from the resident image (what bench.py times)
                 m.stage_resident()
+            fills = poison_all(ms)
             for m in ms:
                 m.convert_resident()
-            for m in ms:
-                assert_pool_matches(m, 0, shards, recs, flags=flags)
+            for i, (m, fill) in enumerate(zip(ms, fills)):
+                helpers.assert_pool_exact(m, 0, exp, mask, fill, f"{os.path.basename(path)} rank {i} of {n}, resident")
         finally:
             for m in ms:
                 m.release()
@@ -605,18 +652,22 @@ def test_virtual_ranks_broadcast_on_one_gpu(pool, tmp_path, n):
 
 def _exchange_on_virtual_ranks(pool, path, n, shards, recs, flags):
     ms = _virtual_ranks(pool, path, gpupool.MODE_SCATTER, n, flags)
+    want = [expected_exact(shards, recs, gpupool.MODE_SCATTER, 0, n, i) for i in range(n)]
+    name = os.path.basename(path)
     try:
+        fills = poison_all(ms)
         for m in ms:
             m.load_part()
         for i, m in enumerate(ms):
-            assert_pool_matches(m, 0, shards, recs, mode=gpupool.MODE_SCATTER, n_parts=n, part=i)
+            helpers.assert_pool_exact(m, 0, *want[i], fills[i], f"{name} rank {i} of {n}")
         if flags:
             for m in ms:
                 m.stage_resident()
+            fills = poison_all(ms)
             for m in ms:
                 m.convert_resident()
             for i, m in enumerate(ms):
-                assert_pool_matches(m, 0, shards, recs, mode=gpupool.MODE_SCATTER, n_parts=n, part=i)
+                helpers.assert_pool_exact(m, 0, *want[i], fills[i], f"{name} rank {i} of {n}, resident")
         return [m.stats() for m in ms]
     finally:
         for m in ms:

@@ -165,13 +165,11 @@ def _rank_main(rank, world, port, paths, out_dir):
                         assert np.array_equal(got[a:b], exp[a:b]), f"rank {rank}: {p['name']} differs"
                     # resident-image path (what bench.py times) must give the same pools
                     m.stage_resident()
+                    fill = helpers.poison(m, rank)  # before the barrier: every rank's launch stores into this pool
                     dist.barrier()
                     m.convert_resident()
                     dist.barrier()
-                    got = m.read(rank, 0, len(exp))
-                    for p in plan:
-                        a, b = p["pool_offset"], p["pool_offset"] + p["nbytes"]
-                        assert np.array_equal(got[a:b], exp[a:b]), f"rank {rank}: {p['name']} differs after resident convert"
+                    helpers.assert_pool_exact(m, rank, exp, helpers.expected_mask(plan, len(exp)), fill, f"rank {rank} after resident convert")
                     dist.barrier()
                     m.peer_detach_all()
                 finally:

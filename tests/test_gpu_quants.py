@@ -9,7 +9,8 @@ import pytest
 
 from kukeon_b200 import gpupool
 from oracle import oracle
-from tests.test_gpu_load import _virtual_ranks, assert_pool_matches, load_and_check
+from tests import helpers
+from tests.test_gpu_load import _virtual_ranks, assert_pool_matches, expected_exact, load_and_check, poison_all
 from tests.test_plan import F4_MIX, f4_tensors
 from tools import synth
 
@@ -195,7 +196,23 @@ def test_pull_fan_out_virtual_ranks_on_one_gpu(pool, tmp_path, n):
     for path in (d, g):
         shards, recs = oracle.index_path(path)
         ms = _pull_ranks(pool, path, n)
+        exp, mask = expected_exact(shards, recs)
+        name = os.path.basename(path)
+
+        def check(fills, what):
+            # Stage 2 copies each peer's whole pool range [pool_lo, pool_hi) from its slice buffer, gaps between placements included, and
+            # nothing ever writes a slice buffer's gap bytes: inside the peers' ranges (not the rank's own) the gaps may change.  That is
+            # the only exception; every placement and every other gap byte is checked.
+            ranges = [next((q["pool_lo"], q["pool_hi"]) for q in m.stats()["parts"]) for m in ms]
+            for i, m in enumerate(ms):
+                peer_range = np.zeros(len(exp), bool)
+                for j, (lo, hi) in enumerate(ranges):
+                    if j != i:
+                        peer_range[lo:hi] = True
+                helpers.assert_pool_exact(m, 0, exp, mask, fills[i], f"{name} PULL rank {i} of {n}, {what}", may_rewrite=peer_range & ~mask)
+
         try:
+            fills = poison_all(ms)
             for m in ms:
                 m.load_part()
                 assert not m.info()["loaded"]
@@ -204,16 +221,15 @@ def test_pull_fan_out_virtual_ranks_on_one_gpu(pool, tmp_path, n):
                 assert m.info()["loaded"]
             if ms[0].stats()["parts"] and ms[1].stats()["parts"][0]["out_bytes"] >= 4096:
                 assert ms[0].probe_peer(1, gpupool.BUF_SLICE, 1 << 20) > 0.0  # copy-engine read of rank 1's attached slice buffer (here: the same GPU)
-            for m in ms:
-                assert_pool_matches(m, 0, shards, recs)
+            check(fills, "streaming load")
             for m in ms:  # again through the resident image (what bench.py times)
                 m.stage_resident()
+            fills = poison_all(ms)
             for m in ms:
                 m.convert_resident()
             for m in ms:
                 m.convert_local()
-            for m in ms:
-                assert_pool_matches(m, 0, shards, recs)
+            check(fills, "resident")
         finally:
             for m in ms:
                 m.release()
@@ -299,9 +315,11 @@ def test_nvls_broadcast_single_process(native, tmp_path):
             with pytest.raises(gpupool.ErrUnsupported, match="cudaIpcMemHandle"):
                 m.export(0)
             m.stage_resident()
+            fills = [helpers.poison(m, dev) for dev in range(n)]
             m.convert_resident()
+            exp, mask = expected_exact(shards, recs)
             for dev in range(n):
-                assert_pool_matches(m, dev, shards, recs)
+                helpers.assert_pool_exact(m, dev, exp, mask, fills[dev], f"NVLS device {dev}, resident")
         finally:
             m.release()
         m = pl.load(g, mode=gpupool.MODE_BROADCAST, fanout=gpupool.FANOUT_NVLS)

@@ -5,9 +5,9 @@ import os
 import socket
 import sys
 
-import numpy as np
 import pytest
 
+from tests import helpers
 from tools import synth
 
 pytestmark = pytest.mark.gpu
@@ -23,11 +23,8 @@ def _free_port():
     return p
 
 
-def _check(m, rank, exp, plan, what):
-    got = m.read(0, 0, len(exp))
-    for p in plan:
-        a, b = p["pool_offset"], p["pool_offset"] + p["nbytes"]
-        assert np.array_equal(got[a:b], exp[a:b]), f"rank {rank} {what}: {p['name']} differs"
+def _check(m, rank, exp, plan, fill, what):
+    helpers.assert_pool_exact(m, 0, exp, helpers.expected_mask(plan, len(exp)), fill, f"rank {rank} {what}")
 
 
 def _rank_main(rank, port, path, out_dir):
@@ -50,20 +47,22 @@ def _rank_main(rank, port, path, out_dir):
                     if r != rank:
                         m.peer_attach_buffer(r, gp.BUF_RAW, h)
                 dist.barrier()
+                fill = helpers.poison(m, 0)  # stage 2 writes only the own pool
                 m.load_part()  # stage 1: own part into the own raw image and, by the COPY fan-out, into the peer's
                 assert not m.info()["loaded"]
                 dist.barrier()
                 m.convert_local()  # stage 2: the whole gathered image into the own pool
                 assert m.info()["loaded"]
-                _check(m, rank, exp, plan, "RAW")
+                _check(m, rank, exp, plan, fill, "RAW")
                 # resident measurement path: stage the own part again, time the fan-out alone, convert again
                 m.stage_resident()
+                fill = helpers.poison(m, 0)
                 dist.barrier()
                 ms, per = m.convert_resident()
                 assert len(per) == 1 and ms >= 0.0  # one fan-out launch over this rank's chunks
                 dist.barrier()
                 m.convert_local()
-                _check(m, rank, exp, plan, "RAW after the resident fan-out")
+                _check(m, rank, exp, plan, fill, "RAW after the resident fan-out")
                 dist.barrier()
                 m.peer_detach_all()
             finally:
