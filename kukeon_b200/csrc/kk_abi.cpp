@@ -199,7 +199,7 @@ int kk_export_buffer(kk_model* m, int device, int which, void* h) {
     bool by_ptr;
     if (!buf_kind(which, kind, by_ptr) || (kind == kk::kPeerPool && by_ptr)) kk::fail(KK_EINVAL, "unknown buffer kind %d", which);
     if (kind == kk::kPeerPool) {
-      if (m->nvls) kk::fail(KK_EUNSUPPORTED, "pools of a KK_FANOUT_NVLS model cannot be exported over CUDA IPC");
+      if (m->pools[(size_t)li].is_nvls()) kk::fail(KK_EUNSUPPORTED, "pools of a KK_FANOUT_NVLS model cannot be exported over CUDA IPC");
       kk::model_pool_ipc_handle(m, li, h);
     } else if (kind == kk::kPeerRaw) {
       kk::model_export_raw(m, li, h);
@@ -236,7 +236,7 @@ int kk_model_get_info(kk_model* m, kk_model_info* o) {
     o->n_shards = m->plan.index.shards.size();
     o->file_bytes = m->plan.file_bytes;
     uint64_t pb = 0;
-    for (auto b : m->pool_bytes) pb = b > pb ? b : pb;
+    for (auto& pool : m->pools) pb = pool.bytes > pb ? pool.bytes : pb;
     o->pool_bytes = pb;
     o->n_devices = (int32_t)m->dev_idx.size();
     for (size_t i = 0; i < m->dev_idx.size(); ++i) o->devices[i] = m->ctx->devs[(size_t)m->dev_idx[i]].ordinal;
@@ -306,8 +306,9 @@ int kk_export(kk_model* m, int device, void* ipc_handle_64B, char* manifest_json
       memcpy(manifest_json, s.c_str(), s.size() + 1);
     }
     if (ipc_handle_64B) {
-      if (m->nvls) kk::fail(KK_EUNSUPPORTED, "pools of a KK_FANOUT_NVLS model are VMM allocations: there is no cudaIpcMemHandle for them (export the manifest only, or load with KK_FANOUT_P2P)");
-      if (!m->vmm.empty()) kk::fail(KK_EUNSUPPORTED, "pools of a KK_CFG_VMM_POOLS context are VMM allocations: there is no cudaIpcMemHandle for them, export the file descriptor (kk_export_fd)");
+      const kk::Pool& pool = m->pools[(size_t)li];
+      if (pool.is_nvls()) kk::fail(KK_EUNSUPPORTED, "pools of a KK_FANOUT_NVLS model are VMM allocations: there is no cudaIpcMemHandle for them (export the manifest only, or load with KK_FANOUT_P2P)");
+      if (pool.vmm) kk::fail(KK_EUNSUPPORTED, "pools of a KK_CFG_VMM_POOLS context are VMM allocations: there is no cudaIpcMemHandle for them, export the file descriptor (kk_export_fd)");
       kk::model_pool_ipc_handle(m, li, ipc_handle_64B);
     }
   });
@@ -323,9 +324,10 @@ int kk_export_fd(kk_model* m, int device, int* fd_out, uint64_t* mapped_bytes) {
     need(fd_out, "fd_out");
     *fd_out = -1;
     int li = kk::model_local_device(m, device);
-    if (m->vmm.size() <= (size_t)li || !m->vmm[(size_t)li]) kk::fail(KK_EUNSUPPORTED, "this pool is a cudaMalloc allocation: open the context with KK_CFG_VMM_POOLS to export file descriptors");
-    *fd_out = m->vmm[(size_t)li]->export_fd();
-    if (mapped_bytes) *mapped_bytes = m->vmm[(size_t)li]->bytes();
+    const kk::VmmAlloc* vmm = m->pools[(size_t)li].vmm.get();
+    if (!vmm) kk::fail(KK_EUNSUPPORTED, "this pool is a cudaMalloc allocation: open the context with KK_CFG_VMM_POOLS to export file descriptors");
+    *fd_out = vmm->export_fd();
+    if (mapped_bytes) *mapped_bytes = vmm->bytes();
   });
 }
 
@@ -337,14 +339,8 @@ int kk_import_fd(int fd, int device, uint64_t mapped_bytes, uint32_t flags, void
     *out = nullptr;
     if (fd < 0 || mapped_bytes == 0) kk::fail(KK_EINVAL, "bad fd / size");
     if (flags & ~KK_IMPORT_READONLY) kk::fail(KK_EINVAL, "unknown import flags 0x%x", flags);
-    kk_import* im = new kk_import;
-    try {
-      im->im = kk::vmm_import_fd(fd, device, mapped_bytes, (flags & KK_IMPORT_READONLY) != 0);
-    } catch (...) {
-      delete im;
-      throw;
-    }
-    *dev_ptr = (void*)(uintptr_t)im->im.va;
+    kk_import* im = new kk_import{kk::vmm_import_fd(fd, device, mapped_bytes, (flags & KK_IMPORT_READONLY) != 0)};
+    *dev_ptr = im->im.map.ptr();
     *out = im;
   });
 }
@@ -352,7 +348,6 @@ int kk_import_fd(int fd, int device, uint64_t mapped_bytes, uint32_t flags, void
 int kk_import_close(kk_import* im) {
   return guard([&] {
     need(im, "import");
-    kk::vmm_import_close(im->im);
     delete im;
   });
 }
@@ -361,8 +356,8 @@ int kk_pool_ptr(kk_model* m, int device, void** p, uint64_t* nbytes) {
   return guard([&] {
     need(m, "model");
     int li = kk::model_local_device(m, device);
-    if (p) *p = m->pools[(size_t)li];
-    if (nbytes) *nbytes = m->pool_bytes[(size_t)li];
+    if (p) *p = m->pools[(size_t)li].ptr;
+    if (nbytes) *nbytes = m->pools[(size_t)li].bytes;
   });
 }
 
@@ -398,9 +393,10 @@ int kk_read(kk_model* m, int device, uint64_t off, uint64_t nbytes, void* host_d
     int li = kk::model_local_device(m, device);
     if (nbytes == 0) return;
     need(host_dst, "host_dst");
-    if (off > m->pool_bytes[(size_t)li] || nbytes > m->pool_bytes[(size_t)li] - off) kk::fail(KK_EINVAL, "range outside the pool");
+    const kk::Pool& pool = m->pools[(size_t)li];
+    if (off > pool.bytes || nbytes > pool.bytes - off) kk::fail(KK_EINVAL, "range outside the pool");
     KK_CUDA(cudaSetDevice(device));
-    KK_CUDA(cudaMemcpy(host_dst, m->pools[(size_t)li] + off, nbytes, cudaMemcpyDeviceToHost));
+    KK_CUDA(cudaMemcpy(host_dst, pool.ptr + off, nbytes, cudaMemcpyDeviceToHost));
   });
 }
 
@@ -409,16 +405,17 @@ int kk_checksum(kk_model* m, int device, uint64_t off, uint64_t nbytes, uint64_t
     need(m, "model");
     need(out, "out");
     int li = kk::model_local_device(m, device);
-    if (off > m->pool_bytes[(size_t)li] || nbytes > m->pool_bytes[(size_t)li] - off) kk::fail(KK_EINVAL, "range outside the pool");
+    const kk::Pool& pool = m->pools[(size_t)li];
+    if (off > pool.bytes || nbytes > pool.bytes - off) kk::fail(KK_EINVAL, "range outside the pool");
     if (off % 8) kk::fail(KK_EINVAL, "pool_offset must be a multiple of 8");
     kk::Device& d = m->ctx->devs[(size_t)m->dev_idx[(size_t)li]];
     KK_CUDA(cudaSetDevice(device));
     // the accumulator lives in the device's scratch words: a cudaMalloc + cudaFree pair per call synchronises the whole device and, next to a
     // 16 GB pool, stalls for tens of milliseconds every few calls
     std::lock_guard<std::mutex> one(*d.sum_mu);
-    unsigned long long* acc = (unsigned long long*)(d.sched + 32);
+    unsigned long long* acc = (unsigned long long*)(d.sched.get<uint32_t>() + 32);
     KK_CUDA(cudaMemsetAsync(acc, 0, 8, d.stream));
-    KK_CUDA(kk::launch_checksum(m->pools[(size_t)li] + off, nbytes, acc, d.sm_count, d.stream));
+    KK_CUDA(kk::launch_checksum(pool.ptr + off, nbytes, acc, d.sm_count, d.stream));
     unsigned long long h = 0;
     KK_CUDA(cudaMemcpyAsync(&h, acc, 8, cudaMemcpyDeviceToHost, d.stream));
     KK_CUDA(cudaStreamSynchronize(d.stream));
@@ -459,30 +456,21 @@ int kk_probe_hbm(kk_ctx* ctx, int device, int kind, uint64_t nbytes, float* ms) 
     if (!d) kk::fail(KK_EINVAL, "device %d is not part of this context", device);
     nbytes &= ~(uint64_t)15;
     if (nbytes == 0) kk::fail(KK_EINVAL, "probe needs at least 16 bytes");
-    KK_CUDA(cudaSetDevice(device));
-    struct Buf {
-      void* p = nullptr;
-      ~Buf() { if (p) cudaFree(p); }
-    } dst, src;
-    struct Ev {
-      cudaEvent_t e = nullptr;
-      ~Ev() { if (e) cudaEventDestroy(e); }
-    } e0, e1;
-    if (cudaMalloc(&dst.p, nbytes) != cudaSuccess) { cudaGetLastError(); kk::fail(KK_ENOMEM, "device %d: cudaMalloc(%llu) for the probe failed", device, (unsigned long long)nbytes); }
+    kk::DevBuf dst(device, nbytes, "the probe"), src;
     if (kind == KK_PROBE_COPY) {
-      if (cudaMalloc(&src.p, nbytes) != cudaSuccess) { cudaGetLastError(); kk::fail(KK_ENOMEM, "device %d: cudaMalloc(%llu) for the probe failed", device, (unsigned long long)nbytes); }
-      KK_CUDA(cudaMemsetAsync(src.p, 0x3C, nbytes, d->stream));
+      src = kk::DevBuf(device, nbytes, "the probe");
+      KK_CUDA(cudaMemsetAsync(src.get(), 0x3C, nbytes, d->stream));
     }
-    KK_CUDA(cudaEventCreate(&e0.e));
-    KK_CUDA(cudaEventCreate(&e1.e));
+    kk::EventSet ev(2);
+    ev.create_all();
     for (int pass = 0; pass < 2; ++pass) {  // pass 0 warms up (first touch of the scratch pages), pass 1 is timed
-      if (pass) KK_CUDA(cudaEventRecord(e0.e, d->stream));
-      if (kind == KK_PROBE_WRITE) KK_CUDA(kk::launch_fill((uint8_t*)dst.p, nbytes, d->sm_count, d->stream));
-      else KK_CUDA(kk::launch_ldg_copy((const uint8_t*)src.p, (uint8_t*)dst.p, nbytes, d->sm_count, d->stream));
-      if (pass) KK_CUDA(cudaEventRecord(e1.e, d->stream));
+      if (pass) KK_CUDA(cudaEventRecord(ev[0], d->stream));
+      if (kind == KK_PROBE_WRITE) KK_CUDA(kk::launch_fill(dst.get(), nbytes, d->sm_count, d->stream));
+      else KK_CUDA(kk::launch_ldg_copy(src.get(), dst.get(), nbytes, d->sm_count, d->stream));
+      if (pass) KK_CUDA(cudaEventRecord(ev[1], d->stream));
     }
     KK_CUDA(cudaStreamSynchronize(d->stream));
-    KK_CUDA(cudaEventElapsedTime(ms, e0.e, e1.e));
+    KK_CUDA(cudaEventElapsedTime(ms, ev[0], ev[1]));
   });
 }
 
@@ -491,20 +479,9 @@ int kk_device_identity(int device, char* pci_bus_id, size_t pci_cap, char* uuid,
     int count = 0;
     if (cudaGetDeviceCount(&count) != cudaSuccess) { cudaGetLastError(); kk::fail(KK_ECUDA, "no usable CUDA device"); }
     if (device < 0 || device >= count) kk::fail(KK_EINVAL, "device %d out of range (0..%d)", device, count - 1);
-    if (pci_bus_id) {
-      if (pci_cap < 16) kk::fail(KK_ERANGE, "pci_bus_id needs 16 bytes");
-      KK_CUDA(cudaDeviceGetPCIBusId(pci_bus_id, (int)pci_cap, device));
-      for (char* c = pci_bus_id; *c; ++c)
-        if (*c >= 'A' && *c <= 'F') *c = (char)(*c - 'A' + 'a');  // /proc/driver/nvidia/gpus/ uses lower case
-    }
-    if (uuid) {
-      if (uuid_cap < 41) kk::fail(KK_ERANGE, "uuid needs 41 bytes");
-      cudaDeviceProp pr;
-      KK_CUDA(cudaGetDeviceProperties(&pr, device));
-      const unsigned char* b = (const unsigned char*)pr.uuid.bytes;
-      snprintf(uuid, uuid_cap, "GPU-%02x%02x%02x%02x-%02x%02x-%02x%02x-%02x%02x-%02x%02x%02x%02x%02x%02x", b[0], b[1], b[2], b[3], b[4], b[5], b[6], b[7], b[8],
-               b[9], b[10], b[11], b[12], b[13], b[14], b[15]);
-    }
+    if (pci_bus_id && pci_cap < 16) kk::fail(KK_ERANGE, "pci_bus_id needs 16 bytes");
+    if (uuid && uuid_cap < 41) kk::fail(KK_ERANGE, "uuid needs 41 bytes");
+    kk::device_identity(device, pci_bus_id, pci_cap, uuid, uuid_cap);
   });
 }
 

@@ -22,12 +22,6 @@
 #include "kk_json.hpp"
 #include "kk_read.hpp"
 
-// A host test that #includes this file whole, to reach the functions of its anonymous namespace, links the library's other objects but not
-// kk_read.o: such a translation unit compiles the read path in with this file.  The library itself links kk_read.o.
-#if __INCLUDE_LEVEL__ > 0
-#include "kk_read.cpp"
-#endif
-
 namespace kk {
 
 namespace {
@@ -40,8 +34,12 @@ double now_s() {
 std::vector<int> numa_cpus_of_device(int ordinal) {
   std::vector<int> cpus;
   char bdf[32] = {0};
-  if (cudaDeviceGetPCIBusId(bdf, sizeof bdf, ordinal) != cudaSuccess) { cudaGetLastError(); return cpus; }
-  for (char* c = bdf; *c; ++c) *c = (char)tolower(*c);
+  try {
+    device_identity(ordinal, bdf, sizeof bdf, nullptr, 0);
+  } catch (const Error&) {
+    cudaGetLastError();
+    return cpus;
+  }
   char path[256];
   snprintf(path, sizeof path, "/sys/bus/pci/devices/%s/numa_node", bdf);
   FILE* f = fopen(path, "r");
@@ -89,38 +87,11 @@ struct ErrorSink {
   }
 };
 
-// CUDA events / scratch device memory that must not leak when a KK_CUDA check throws half way through a function.
-struct EventSet {
-  std::vector<cudaEvent_t> ev;
-  explicit EventSet(size_t n = 0) : ev(n, nullptr) {}
-  cudaEvent_t& operator[](size_t i) { return ev[i]; }
-  size_t size() const { return ev.size(); }
-  void create_all() {
-    for (auto& e : ev) KK_CUDA(cudaEventCreate(&e));
-  }
-  ~EventSet() {
-    for (auto e : ev)
-      if (e) cudaEventDestroy(e);
-  }
-  EventSet(const EventSet&) = delete;
-  EventSet& operator=(const EventSet&) = delete;
-  EventSet(EventSet&& o) noexcept : ev(std::move(o.ev)) { o.ev.clear(); }
-};
-struct DevScratch {
-  void* p = nullptr;
-  ~DevScratch() {
-    if (p) cudaFree(p);
-  }
-};
-
-// Device copy of a segment table on the current device (nullptr for an empty table); the caller frees it.
-KKSeg* upload_segs(const std::vector<KKSeg>& segs) {
-  KKSeg* d = nullptr;
-  if (segs.empty()) return d;
-  KK_CUDA(cudaMalloc((void**)&d, segs.size() * sizeof(KKSeg)));
-  const cudaError_t e = cudaMemcpy(d, segs.data(), segs.size() * sizeof(KKSeg), cudaMemcpyHostToDevice);
-  if (e != cudaSuccess) cudaFree(d);
-  KK_CUDA(e);
+// Device copy of a segment table on device `ordinal` (empty for an empty table).
+DevBuf upload_segs(int ordinal, const std::vector<KKSeg>& segs) {
+  if (segs.empty()) return DevBuf();
+  DevBuf d(ordinal, segs.size() * sizeof(KKSeg), "a segment table");
+  KK_CUDA(cudaMemcpy(d.get(), segs.data(), segs.size() * sizeof(KKSeg), cudaMemcpyHostToDevice));
   return d;
 }
 
@@ -222,7 +193,7 @@ void fill_dsts(kk_model* m, int li, ConvertLaunch& L) {
   L.n_dst = 0;
   L.flags = 0;
   for (auto& d : L.dst) d = nullptr;
-  L.dst[L.n_dst++] = m->pools[(size_t)li];
+  L.dst[L.n_dst++] = m->pools[(size_t)li].ptr;
   L.n_xdst = 0;
   for (auto& d : L.xdst) d = nullptr;
   if (m->plan.mode == KK_MODE_SCATTER && (m->plan.flags & KK_LOAD_SCATTER_EXCHANGE) && m->plan.n_parts > 1) {
@@ -230,8 +201,8 @@ void fill_dsts(kk_model* m, int li, ConvertLaunch& L) {
     const int n = m->plan.n_parts;
     for (int j = 0; j < n; ++j) {
       uint8_t* p = nullptr;
-      if (m->opts.part_count > 1) p = (j == m->opts.part_index) ? m->pools[0] : (uint8_t*)m->peer[kPeerPool][j].ptr;
-      else if (m->ctx->peer_ok) p = m->pools[(size_t)j];
+      if (m->opts.part_count > 1) p = (j == m->opts.part_index) ? m->pools[0].ptr : (uint8_t*)m->peer[kPeerPool][j].ptr;
+      else if (m->ctx->peer_ok) p = m->pools[(size_t)j].ptr;
       if (!p) fail(KK_ESTATE, "KK_LOAD_SCATTER_EXCHANGE: the pool of rank %d is not reachable (attach it with kk_peer_attach, or enable peer access)", j);
       L.xdst[j] = p;
     }
@@ -244,7 +215,7 @@ void fill_dsts(kk_model* m, int li, ConvertLaunch& L) {
     return;
   }
   if (is_pull(m)) {  // stage 1 of a pull load: the same bytes into the slice buffer the peers will read (pool offset -> slice_buf - slice_base)
-    if (m->slice_buf) L.dst[L.n_dst++] = (uint8_t*)((uintptr_t)m->slice_buf - (uintptr_t)m->slice_base);
+    if (m->slice_buf) L.dst[L.n_dst++] = (uint8_t*)((uintptr_t)m->slice_buf.get() - (uintptr_t)m->slice_base);
     return;
   }
   if (m->plan.mode != KK_MODE_BROADCAST || m->opts.fanout == KK_FANOUT_NONE) {
@@ -256,7 +227,7 @@ void fill_dsts(kk_model* m, int li, ConvertLaunch& L) {
       if (b.ptr) L.dst[L.n_dst++] = (uint8_t*)b.ptr;
   } else if (m->ctx->peer_ok) {
     for (size_t j = 0; j < m->pools.size(); ++j)
-      if ((int)j != li) L.dst[L.n_dst++] = m->pools[j];
+      if ((int)j != li) L.dst[L.n_dst++] = m->pools[j].ptr;
   }
   pad_dsts_for_test(L);
 }
@@ -270,8 +241,8 @@ void fill_raw_dsts(kk_model* m, int li, ConvertLaunch& L) {
     for (auto& b : m->peer[kPeerRaw])
       if (b.ptr) L.dst[L.n_dst++] = (uint8_t*)b.ptr;
   } else {
-    for (size_t j = 0; j < m->raw.size(); ++j)
-      if ((int)j != li) L.dst[L.n_dst++] = m->raw[j].image;
+    for (size_t j = 0; j < m->images.size(); ++j)
+      if ((int)j != li) L.dst[L.n_dst++] = m->images[j].image.get();
   }
 }
 
@@ -340,7 +311,7 @@ void convert_part(kk_model* m, int li, int part, const FdSet& fds) {
   if (pp.chunks.empty()) return;
   const int sm_count = m->ctx->devs[(size_t)m->dev_idx[(size_t)li]].sm_count;
   const bool zerocopy = (m->ctx->cfg.flags & KK_CFG_ZEROCOPY) != 0;
-  const KKSeg* d_segs = m->d_segs[(size_t)li] + seg_base_of(m->plan, part);
+  const KKSeg* d_segs = m->d_segs[(size_t)li].get<KKSeg>() + seg_base_of(m->plan, part);
   ConvertLaunch base{};
   fill_dsts(m, li, base);
   stream_part(m, li, part, fds, true, [&](Reader& rd, Slot& s, size_t ci) {
@@ -348,13 +319,13 @@ void convert_part(kk_model* m, int li, int part, const FdSet& fds) {
     ConvertLaunch L = base;
     L.src = s.pinned;
     if (!zerocopy) {
-      KK_CUDA(cudaMemcpyAsync(s.dev, s.pinned, ch.buf_bytes, cudaMemcpyHostToDevice, rd.stream));
-      L.src = s.dev;
+      KK_CUDA(cudaMemcpyAsync(s.dev.get(), s.pinned, ch.buf_bytes, cudaMemcpyHostToDevice, rd.stream));
+      L.src = s.dev.get();
     }
     L.segs = d_segs + ch.seg_begin;
     L.n_segs = ch.seg_count;
     L.n_tiles = ch.n_tiles;
-    L.sched = rd.sched;
+    L.sched = rd.sched.get<uint32_t>();
     KK_CUDA(launch_convert(L, sm_count, rd.stream));
   });
 }
@@ -366,20 +337,20 @@ void raw_stage1(kk_model* m, int li, const FdSet& fds) {
   const PartPlan& pp = m->plan.parts[(size_t)part];
   if (pp.chunks.empty()) return;
   const int sm_count = m->ctx->devs[(size_t)m->dev_idx[(size_t)li]].sm_count;
-  kk_model::Raw& R = m->raw[(size_t)li];
+  const DeviceImage& R = m->images[(size_t)li];
   ConvertLaunch base{};
   fill_raw_dsts(m, li, base);
   if (base.n_dst > 0 && !m->ctx->peer_ok && m->opts.part_count <= 1) fail(KK_EUNSUPPORTED, "KK_FANOUT_RAW needs peer access between the context's devices");
   stream_part(m, li, part, fds, true, [&](Reader& rd, Slot& s, size_t ci) {
     const Chunk& ch = pp.chunks[ci];
-    KK_CUDA(cudaMemcpyAsync(R.image + m->img_off[(size_t)part][ci], s.pinned, ch.buf_bytes, cudaMemcpyHostToDevice, rd.stream));
+    KK_CUDA(cudaMemcpyAsync(R.image.get() + m->img_off[(size_t)part][ci], s.pinned, ch.buf_bytes, cudaMemcpyHostToDevice, rd.stream));
     if (base.n_dst == 0) return;
     ConvertLaunch L = base;
-    L.src = R.image;
-    L.segs = R.d_copy_segs + m->chunk_base[(size_t)part] + ci;
+    L.src = R.image.get();
+    L.segs = R.copy_segs.get<KKSeg>() + m->chunk_base[(size_t)part] + ci;
     L.n_segs = 1;
     L.n_tiles = (uint32_t)kk_seg_tiles(KK_OP_COPY, align_up(ch.buf_bytes, 16), 0);
-    L.sched = rd.sched;
+    L.sched = rd.sched.get<uint32_t>();
     KK_CUDA(launch_convert(L, sm_count, rd.stream));
   });
 }
@@ -411,38 +382,25 @@ void setup_raw(kk_model* m) {
       copy_segs.push_back(cs);
     }
   }
-  m->raw.resize(m->dev_idx.size());
+  m->images.resize(m->dev_idx.size());
   for (size_t li = 0; li < m->dev_idx.size(); ++li) {
-    Device& d = m->ctx->devs[(size_t)m->dev_idx[li]];
-    KK_CUDA(cudaSetDevice(d.ordinal));
-    auto& R = m->raw[li];
-    R.bytes = align_up(im.bytes ? im.bytes : 256, 2u << 20);  // 2 MiB multiples: cheap to map over CUDA IPC (see the slice buffer in model_load)
-    cudaError_t e = cudaMalloc((void**)&R.image, R.bytes);
-    if (e != cudaSuccess) { cudaGetLastError(); R.image = nullptr; fail(KK_ENOMEM, "device %d: cudaMalloc(%llu) for the raw image failed", d.ordinal, (unsigned long long)R.bytes); }
-    R.d_copy_segs = upload_segs(copy_segs);
-    R.d_conv_segs = upload_segs(im.segs);
-    R.conv_launches = im.launches;
+    const int ordinal = m->ctx->devs[(size_t)m->dev_idx[li]].ordinal;
+    DeviceImage& R = m->images[li];
+    // 2 MiB multiples: cheap to map over CUDA IPC (see the slice buffer in model_load)
+    R.image = DevBuf(ordinal, align_up(im.bytes ? im.bytes : 256, 2u << 20), "the raw image");
+    R.copy_segs = upload_segs(ordinal, copy_segs);
+    R.segs = upload_segs(ordinal, im.segs);
+    R.launches = im.launches;
   }
-}
-
-void free_raw(kk_model* m) {
-  for (size_t li = 0; li < m->raw.size(); ++li) {
-    auto& R = m->raw[li];
-    cudaSetDevice(m->ctx->devs[(size_t)m->dev_idx[li]].ordinal);
-    if (R.image) cudaFree(R.image);
-    if (R.d_copy_segs) cudaFree(R.d_copy_segs);
-    if (R.d_conv_segs) cudaFree(R.d_conv_segs);
-  }
-  m->raw.clear();
 }
 
 // The launches over a device image, each with base's destinations.
-std::vector<ConvertLaunch> image_launches(const ConvertLaunch& base, const uint8_t* image, const KKSeg* d_segs, const std::vector<ImageLaunch>& launches) {
+std::vector<ConvertLaunch> image_launches(const ConvertLaunch& base, const DeviceImage& im) {
   std::vector<ConvertLaunch> out;
-  for (auto& la : launches) {
+  for (auto& la : im.launches) {
     ConvertLaunch L = base;
-    L.src = image;
-    L.segs = d_segs + la.seg_begin;
+    L.src = im.image.get();
+    L.segs = im.segs.get<KKSeg>() + la.seg_begin;
     L.n_segs = la.n_segs;
     L.n_tiles = la.n_tiles;
     out.push_back(L);
@@ -463,7 +421,7 @@ float time_launches(kk_model* m, std::vector<std::vector<ConvertLaunch>>& launch
     evs[li].create_all();
     KK_CUDA(cudaEventRecord(evs[li][0], dev.stream));
     for (size_t k = 0; k < launches[li].size(); ++k) {
-      launches[li][k].sched = dev.sched;
+      launches[li][k].sched = dev.sched.get<uint32_t>();
       KK_CUDA(launch_convert(launches[li][k], dev.sm_count, dev.stream));
       KK_CUDA(cudaEventRecord(evs[li][k + 1], dev.stream));
     }
@@ -492,8 +450,8 @@ void convert_local_all(kk_model* m, float* ms_total) {
   for (size_t li = 0; li < launches.size(); ++li) {
     ConvertLaunch base{};
     base.n_dst = 1;
-    base.dst[0] = m->pools[li];
-    launches[li] = image_launches(base, m->raw[li].image, m->raw[li].d_conv_segs, m->raw[li].conv_launches);
+    base.dst[0] = m->pools[li].ptr;
+    launches[li] = image_launches(base, m->images[li]);
   }
   const float ms = time_launches(m, launches);
   if (ms_total) *ms_total = ms;
@@ -515,7 +473,7 @@ void pull_slices(kk_model* m, float* ms_total) {
     if (m->part_range[(size_t)r].second > m->part_range[(size_t)r].first) peers.push_back(r);
   }
   std::vector<std::vector<ConvertLaunch>> launches(1);
-  DevScratch table;  // freed after time_launches has waited for the launch that reads it
+  DevBuf table;  // freed after time_launches has waited for the launch that reads it
   if (!peers.empty()) {
     // one src base for the launch: the numerically lowest peer mapping; every segment's src_off is its distance from it
     uintptr_t base = UINTPTR_MAX;
@@ -535,15 +493,14 @@ void pull_slices(kk_model* m, float* ms_total) {
       segs.push_back(sg);
     }
     if (tiles > 0xFFFFFFF0ull) fail(KK_EUNSUPPORTED, "too many tiles for one pull launch");
-    KK_CUDA(cudaSetDevice(m->ctx->devs[(size_t)m->dev_idx[0]].ordinal));
-    table.p = upload_segs(segs);
+    table = upload_segs(m->ctx->devs[(size_t)m->dev_idx[0]].ordinal, segs);
     ConvertLaunch L{};
     L.src = (const uint8_t*)base;
-    L.segs = (const KKSeg*)table.p;
+    L.segs = table.get<KKSeg>();
     L.n_segs = (uint32_t)segs.size();
     L.n_tiles = (uint32_t)tiles;
     L.n_dst = 1;
-    L.dst[0] = m->pools[0];
+    L.dst[0] = m->pools[0].ptr;
     launches[0].push_back(L);
   }
   const float ms = time_launches(m, launches);
@@ -552,7 +509,7 @@ void pull_slices(kk_model* m, float* ms_total) {
 
 // RAW, kernel-stage measurement: stage 1's fan-out without the file reads — one COPY launch over all of local device li's own chunks, from
 // its raw image into every peer image.  table receives the launch's segment table.
-void raw_fanout_launch(kk_model* m, int li, DevScratch& table, std::vector<ConvertLaunch>& out) {
+void raw_fanout_launch(kk_model* m, int li, DevBuf& table, std::vector<ConvertLaunch>& out) {
   ConvertLaunch L{};
   fill_raw_dsts(m, li, L);
   const int part = m->local_parts[(size_t)li];
@@ -569,25 +526,12 @@ void raw_fanout_launch(kk_model* m, int li, DevScratch& table, std::vector<Conve
     tiles += (uint32_t)kk_seg_tiles(KK_OP_COPY, sg.units, 0);
   }
   if (segs.size() > kMaxSegsPerLaunch) fail(KK_EUNSUPPORTED, "too many chunks for one raw fan-out launch");
-  KK_CUDA(cudaSetDevice(m->ctx->devs[(size_t)m->dev_idx[(size_t)li]].ordinal));
-  table.p = upload_segs(segs);
-  L.src = m->raw[(size_t)li].image;
-  L.segs = (const KKSeg*)table.p;
+  table = upload_segs(m->ctx->devs[(size_t)m->dev_idx[(size_t)li]].ordinal, segs);
+  L.src = m->images[(size_t)li].image.get();
+  L.segs = table.get<KKSeg>();
   L.n_segs = (uint32_t)segs.size();
   L.n_tiles = tiles;
   out.push_back(L);
-}
-
-void free_resident(kk_model* m) {
-  for (size_t li = 0; li < m->resident.size(); ++li) {
-    auto& R = m->resident[li];
-    if (R.image || R.d_segs) {
-      cudaSetDevice(m->ctx->devs[(size_t)m->dev_idx[li]].ordinal);
-      if (R.image) cudaFree(R.image);
-      if (R.d_segs) cudaFree(R.d_segs);
-    }
-  }
-  m->resident.clear();
 }
 
 // Close the peer buffers this process opened over CUDA IPC and forget every attached one.
@@ -602,28 +546,9 @@ void close_peers(kk_model* m) {
     }
 }
 
+// Peer mappings close first; the model's buffers and pools go with it (the NVLS object after the pools that alias it).
 void destroy_model(kk_model* m) {
-  kk_ctx* c = m->ctx;
   close_peers(m);
-  free_resident(m);
-  free_raw(m);
-  if (m->slice_buf) {
-    cudaSetDevice(c->devs[(size_t)m->dev_idx[0]].ordinal);
-    cudaFree(m->slice_buf);
-    m->slice_buf = nullptr;
-  }
-  for (size_t i = 0; i < m->pools.size(); ++i) {
-    Device& d = c->devs[(size_t)m->dev_idx[i]];
-    cudaSetDevice(d.ordinal);
-    if (m->pools[i]) {
-      if (!m->nvls && m->vmm.empty()) cudaFree(m->pools[i]);  // NVLS / VMM pools are unmapped and released by their owners below
-      std::lock_guard<std::mutex> g(c->mu);  // model_load checks the budget under the same lock
-      d.pool_in_use -= m->pool_bytes[i];
-    }
-    if (i < m->d_segs.size() && m->d_segs[i]) cudaFree(m->d_segs[i]);
-  }
-  m->nvls.reset();
-  m->vmm.clear();
   delete m;
 }
 
@@ -634,6 +559,29 @@ std::string canon(const std::string& p) {
 }
 
 }  // namespace
+
+Pool::~Pool() {
+  mem = DevBuf();  // the memory before its budget: a load that then passes the budget check must find the memory free
+  vmm.reset();
+  if (!ctx) return;
+  std::lock_guard<std::mutex> g(ctx->mu);  // model_load checks the budget under the same lock
+  dev->pool_in_use -= bytes;
+}
+
+void device_identity(int ordinal, char* bus, size_t bus_cap, char* uuid, size_t uuid_cap) {
+  if (bus) {
+    KK_CUDA(cudaDeviceGetPCIBusId(bus, (int)bus_cap, ordinal));
+    for (char* c = bus; *c; ++c)
+      if (*c >= 'A' && *c <= 'F') *c = (char)(*c - 'A' + 'a');
+  }
+  if (uuid) {
+    cudaDeviceProp pr;
+    KK_CUDA(cudaGetDeviceProperties(&pr, ordinal));
+    const unsigned char* b = (const unsigned char*)pr.uuid.bytes;
+    snprintf(uuid, uuid_cap, "GPU-%02x%02x%02x%02x-%02x%02x-%02x%02x-%02x%02x-%02x%02x%02x%02x%02x%02x", b[0], b[1], b[2], b[3], b[4], b[5], b[6], b[7],
+             b[8], b[9], b[10], b[11], b[12], b[13], b[14], b[15]);
+  }
+}
 
 // ---------------------------------------------------------------------------------------------
 // context
@@ -682,21 +630,21 @@ kk_ctx* ctx_open(const kk_config& cfg_in) {
           KK_CUDA(kernels_init_device());
           d.kernels_ready = true;
           KK_CUDA(cudaStreamCreateWithFlags(&d.stream, cudaStreamNonBlocking));
-          KK_CUDA(cudaMalloc((void**)&d.sched, 256));
-          KK_CUDA(cudaMemset(d.sched, 0, 256));
+          d.sched = DevBuf(d.ordinal, 256, "the scheduling words");
+          KK_CUDA(cudaMemset(d.sched.get(), 0, 256));
           d.numa_cpus = numa_cpus_of_device(d.ordinal);
           d.readers.resize(cfg.n_reader_threads);
           if (!(cfg.flags & KK_CFG_NO_NUMA_PIN)) pin_this_thread(d.numa_cpus);
           for (uint32_t r = 0; r < cfg.n_reader_threads; ++r) {
             Reader& rd = d.readers[r];
             KK_CUDA(cudaStreamCreateWithFlags(&rd.stream, cudaStreamNonBlocking));
-            KK_CUDA(cudaMalloc((void**)&rd.sched, 256));
-            KK_CUDA(cudaMemset(rd.sched, 0, 256));
+            rd.sched = DevBuf(d.ordinal, 256, "the scheduling words");
+            KK_CUDA(cudaMemset(rd.sched.get(), 0, 256));
             uint32_t ns = cfg.n_staging_buffers / cfg.n_reader_threads + (r < cfg.n_staging_buffers % cfg.n_reader_threads ? 1 : 0);
             rd.slots.resize(ns);
             for (auto& s : rd.slots) {
               KK_CUDA(cudaHostAlloc((void**)&s.pinned, c->slot_bytes + 256, cudaHostAllocPortable | cudaHostAllocMapped));
-              if (!(cfg.flags & KK_CFG_ZEROCOPY)) KK_CUDA(cudaMalloc((void**)&s.dev, c->slot_bytes + 256));
+              if (!(cfg.flags & KK_CFG_ZEROCOPY)) s.dev = DevBuf(d.ordinal, c->slot_bytes + 256, "a staging buffer");
               KK_CUDA(cudaEventCreateWithFlags(&s.done, cudaEventDisableTiming));
             }
           }
@@ -753,16 +701,13 @@ void ctx_close(kk_ctx* c) {
     for (auto& rd : d.readers) {
       for (auto& s : rd.slots) {
         if (s.done) cudaEventDestroy(s.done);
-        if (s.dev) cudaFree(s.dev);
         if (s.pinned) cudaFreeHost(s.pinned);
       }
       if (rd.stream) cudaStreamDestroy(rd.stream);
-      if (rd.sched) cudaFree(rd.sched);
     }
     if (d.stream) cudaStreamDestroy(d.stream);
-    if (d.sched) cudaFree(d.sched);
   }
-  delete c;
+  delete c;  // the device buffers go with it
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -878,9 +823,8 @@ kk_model* model_load(kk_ctx* c, const std::string& path, const kk_load_opts& opt
     // concatenated segment table of all parts
     std::vector<KKSeg> all;
     for (auto& pp : m->plan.parts) all.insert(all.end(), pp.segs.begin(), pp.segs.end());
-    m->pools.assign(m->dev_idx.size(), nullptr);
-    m->pool_bytes.assign(m->dev_idx.size(), 0);
-    m->d_segs.assign(m->dev_idx.size(), nullptr);
+    m->pools = std::vector<Pool>(m->dev_idx.size());
+    m->d_segs.resize(m->dev_idx.size());
     if (opts.fanout == KK_FANOUT_NVLS) {
       std::string why;
       if (!plan_allows_multimem(m->plan, &why)) fail(KK_EUNSUPPORTED, "fan-out NVLS: %s", why.c_str());
@@ -894,49 +838,35 @@ kk_model* model_load(kk_ctx* c, const std::string& path, const kk_load_opts& opt
       Device& d = c->devs[(size_t)m->dev_idx[li]];
       KK_CUDA(cudaSetDevice(d.ordinal));
       const uint64_t pb = m->plan.pool_bytes_of_part(m->local_parts[li]);
+      Pool& pool = m->pools[li];
       {
         std::lock_guard<std::mutex> g(c->mu);
         if (c->cfg.pool_bytes_per_device && d.pool_in_use + pb > c->cfg.pool_bytes_per_device)
           fail(KK_ENOMEM, "device %d: pool budget exceeded (%llu in use + %llu > %llu)", d.ordinal, (unsigned long long)d.pool_in_use,
                (unsigned long long)pb, (unsigned long long)c->cfg.pool_bytes_per_device);
         d.pool_in_use += pb;
-        m->pool_bytes[li] = pb;
+        pool.bytes = pb;
+        pool.ctx = c;
+        pool.dev = &d;
       }
-      cudaError_t e = cudaSuccess;
       if (m->nvls) {
-        m->pools[li] = m->nvls->pool(li);  // already allocated, bound and mapped
+        pool.ptr = m->nvls->pool(li);  // already allocated, bound and mapped
       } else if (c->cfg.flags & KK_CFG_VMM_POOLS) {
         // cuMemCreate memory: exported as a POSIX fd (kk_export_fd) that another process maps READ-ONLY, which a cudaIpcMemHandle cannot offer.
         // Mapped read-write here for this device and, in a peer-enabled context, for the other devices (fan-out stores land in it).
         std::vector<int> acc;
         if (c->peer_ok)
           for (auto& dv : c->devs) acc.push_back(dv.ordinal);
-        if (m->vmm.size() < m->dev_idx.size()) m->vmm.resize(m->dev_idx.size());
-        try {
-          m->vmm[li].reset(new VmmAlloc);
-          m->vmm[li]->create(d.ordinal, pb, acc);
-          m->pools[li] = m->vmm[li]->ptr();
-        } catch (...) {
-          m->vmm[li].reset();
-          std::lock_guard<std::mutex> g(c->mu);
-          d.pool_in_use -= pb;
-          m->pool_bytes[li] = 0;
-          throw;
-        }
+        pool.vmm.reset(new VmmAlloc);
+        pool.vmm->create(d.ordinal, pb, acc);
+        pool.ptr = pool.vmm->ptr();
       } else {
         // whole 2 MiB multiples: the driver sub-allocates smaller requests out of shared 2 MiB blocks, and an IPC handle maps the whole block —
         // a pool that owns its blocks outright cannot expose a neighbouring allocation through its handle (round-1 review)
-        e = cudaMalloc((void**)&m->pools[li], align_up(pb ? pb : 1, 2u << 20));
+        pool.mem = DevBuf(d.ordinal, align_up(pb ? pb : 1, 2u << 20), "the pool");
+        pool.ptr = pool.mem.get();
       }
-      if (e != cudaSuccess) {
-        cudaGetLastError();
-        m->pools[li] = nullptr;
-        std::lock_guard<std::mutex> g(c->mu);
-        d.pool_in_use -= pb;
-        m->pool_bytes[li] = 0;
-        fail(KK_ENOMEM, "device %d: cudaMalloc(%llu) for the pool failed: %s", d.ordinal, (unsigned long long)pb, cudaGetErrorString(e));
-      }
-      m->d_segs[li] = upload_segs(all);
+      m->d_segs[li] = upload_segs(d.ordinal, all);
     }
     if (is_raw(m)) setup_raw(m);
     if (is_pull(m)) {
@@ -947,17 +877,15 @@ kk_model* model_load(kk_ctx* c, const std::string& path, const kk_load_opts& opt
       const auto& mine = m->part_range[(size_t)opts.part_index];
       m->slice_base = mine.first & ~(uint64_t)255;
       const uint64_t sb = mine.second > m->slice_base ? mine.second - m->slice_base : 0;
-      KK_CUDA(cudaSetDevice(c->devs[(size_t)m->dev_idx[0]].ordinal));
       // whole 2 MiB multiples, like the pools: cudaIpcOpenMemHandle of such an allocation is far cheaper than of one the driver carved out of
       // shared blocks (at N = 8, seven rounded 16 GB pools map faster than seven 2 GB slice buffers of odd size)
-      cudaError_t se = cudaMalloc((void**)&m->slice_buf, align_up(sb ? sb : 256, 2u << 20));
-      if (se != cudaSuccess) { cudaGetLastError(); m->slice_buf = nullptr; fail(KK_ENOMEM, "cudaMalloc(%llu) for the slice buffer failed", (unsigned long long)sb); }
+      m->slice_buf = DevBuf(c->devs[(size_t)m->dev_idx[0]].ordinal, align_up(sb ? sb : 256, 2u << 20), "the slice buffer");
     }
     m->t_alloc = now_s() - t0;
     if (!(opts.flags & KK_LOAD_DEFER)) {
       do_load(m);
       m->loaded = !((is_raw(m) || is_pull(m)) && multi_proc);
-      if (is_raw(m) && !multi_proc) free_raw(m);  // the gathered file bytes are not needed once the pools are built
+      if (is_raw(m) && !multi_proc) m->images.clear();  // the gathered file bytes are not needed once the pools are built
     }
   } catch (...) {
     {
@@ -978,7 +906,7 @@ kk_model* model_load(kk_ctx* c, const std::string& path, const kk_load_opts& opt
 
 void model_load_part(kk_model* m) {
   std::lock_guard<std::mutex> op(m->op_mu);
-  if (is_raw(m) && m->raw.empty()) fail(KK_ESTATE, "the raw image of this model has been released");
+  if (is_raw(m) && m->images.empty()) fail(KK_ESTATE, "the raw image of this model has been released");
   do_load(m);
   std::lock_guard<std::mutex> g(m->ctx->mu);
   if (!((is_raw(m) || is_pull(m)) && m->opts.part_count > 1)) m->loaded = true;  // multi-process RAW / PULL: loaded after kk_convert_local
@@ -992,7 +920,7 @@ void model_convert_local(kk_model* m, float* ms_total) {
     m->loaded = true;
     return;
   }
-  if (!is_raw(m) || m->raw.empty()) fail(KK_ESTATE, "kk_convert_local only applies to KK_FANOUT_RAW models with a live raw image and to KK_FANOUT_PULL models");
+  if (!is_raw(m) || m->images.empty()) fail(KK_ESTATE, "kk_convert_local only applies to KK_FANOUT_RAW models with a live raw image and to KK_FANOUT_PULL models");
   convert_local_all(m, ms_total);
   std::lock_guard<std::mutex> g(m->ctx->mu);
   m->loaded = true;
@@ -1000,23 +928,23 @@ void model_convert_local(kk_model* m, float* ms_total) {
 }
 
 void model_export_raw(kk_model* m, int li, void* handle_out) {
-  if (!is_raw(m) || m->raw.empty()) fail(KK_ESTATE, "this model has no raw image");
+  if (!is_raw(m) || m->images.empty()) fail(KK_ESTATE, "this model has no raw image");
   KK_CUDA(cudaSetDevice(m->ctx->devs[(size_t)m->dev_idx[(size_t)li]].ordinal));
   cudaIpcMemHandle_t h;
-  KK_CUDA(cudaIpcGetMemHandle(&h, m->raw[(size_t)li].image));
+  KK_CUDA(cudaIpcGetMemHandle(&h, m->images[(size_t)li].image.get()));
   memcpy(handle_out, &h, sizeof h);
 }
 
 void model_export_slice(kk_model* m, void* handle_out, bool as_pointer) {
   if (!is_pull(m) || !m->slice_buf) fail(KK_ESTATE, "this model has no slice buffer (KK_FANOUT_PULL only)");
   if (as_pointer) {
-    void* p = m->slice_buf;
+    void* p = m->slice_buf.get();
     memcpy(handle_out, &p, sizeof p);
     return;
   }
   KK_CUDA(cudaSetDevice(m->ctx->devs[(size_t)m->dev_idx[0]].ordinal));
   cudaIpcMemHandle_t h;
-  KK_CUDA(cudaIpcGetMemHandle(&h, m->slice_buf));
+  KK_CUDA(cudaIpcGetMemHandle(&h, m->slice_buf.get()));
   memcpy(handle_out, &h, sizeof h);
 }
 
@@ -1028,9 +956,9 @@ void model_probe_peer(kk_model* m, int rank, PeerKind kind, uint64_t& nbytes, fl
   if (rank < 0 || rank >= KK_MAX_DEVICES) fail(KK_EINVAL, "bad peer rank %d", rank);
   uint64_t avail = 0;
   if (kind == kPeerPool) {
-    avail = m->pool_bytes.empty() ? 0 : m->pool_bytes[0];
+    avail = m->pools.empty() ? 0 : m->pools[0].bytes;
   } else if (kind == kPeerRaw) {
-    avail = m->raw.empty() ? 0 : m->raw[0].bytes;
+    avail = m->images.empty() ? 0 : m->images[0].image.bytes();
   } else if ((size_t)rank < m->part_range.size()) {
     const auto& pr = m->part_range[(size_t)rank];
     avail = pr.second > (pr.first & ~(uint64_t)255) ? pr.second - (pr.first & ~(uint64_t)255) : 0;
@@ -1044,14 +972,12 @@ void model_probe_peer(kk_model* m, int rank, PeerKind kind, uint64_t& nbytes, fl
   nbytes = std::min(nbytes, avail) & ~(uint64_t)255;
   if (!nbytes) fail(KK_EINVAL, "probe: nothing to copy from rank %d", rank);
   Device& dev = m->ctx->devs[(size_t)m->dev_idx[0]];
-  KK_CUDA(cudaSetDevice(dev.ordinal));
-  DevScratch tmp;
-  if (cudaMalloc(&tmp.p, nbytes) != cudaSuccess) { cudaGetLastError(); fail(KK_ENOMEM, "probe: cudaMalloc(%llu) failed", (unsigned long long)nbytes); }
+  DevBuf tmp(dev.ordinal, nbytes, "the peer probe");
   EventSet ev(2);
   ev.create_all();
-  KK_CUDA(cudaMemcpyAsync(tmp.p, src, nbytes, cudaMemcpyDeviceToDevice, dev.stream));
+  KK_CUDA(cudaMemcpyAsync(tmp.get(), src, nbytes, cudaMemcpyDeviceToDevice, dev.stream));
   KK_CUDA(cudaEventRecord(ev[0], dev.stream));
-  KK_CUDA(cudaMemcpyAsync(tmp.p, src, nbytes, cudaMemcpyDeviceToDevice, dev.stream));
+  KK_CUDA(cudaMemcpyAsync(tmp.get(), src, nbytes, cudaMemcpyDeviceToDevice, dev.stream));
   KK_CUDA(cudaEventRecord(ev[1], dev.stream));
   KK_CUDA(cudaStreamSynchronize(dev.stream));
   KK_CUDA(cudaEventElapsedTime(ms, ev[0], ev[1]));
@@ -1124,7 +1050,7 @@ void model_pool_ipc_handle(kk_model* m, int li, void* handle_out) {
   if (c.empty()) {
     KK_CUDA(cudaSetDevice(m->ctx->devs[(size_t)m->dev_idx[(size_t)li]].ordinal));
     cudaIpcMemHandle_t h;
-    KK_CUDA(cudaIpcGetMemHandle(&h, m->pools[(size_t)li]));
+    KK_CUDA(cudaIpcGetMemHandle(&h, m->pools[(size_t)li].ptr));
     static_assert(sizeof h == KK_IPC_HANDLE_BYTES, "ipc handle size");
     c.assign((const uint8_t*)&h, (const uint8_t*)&h + sizeof h);
   }
@@ -1147,21 +1073,14 @@ static std::string build_manifest(kk_model* m, int li) {
   // "device" is the ordinal in THIS process (diagnostics only); a consumer in another process or container finds the GPU by its UUID / PCI bus id
   const int ordinal = m->ctx->devs[(size_t)m->dev_idx[(size_t)li]].ordinal;
   char bus[32] = "", uuid[48] = "";
-  {
-    cudaDeviceProp pr;
-    if (cudaDeviceGetPCIBusId(bus, (int)sizeof bus, ordinal) != cudaSuccess) { cudaGetLastError(); bus[0] = 0; }
-    for (char* c = bus; *c; ++c)
-      if (*c >= 'A' && *c <= 'F') *c = (char)(*c - 'A' + 'a');
-    if (cudaGetDeviceProperties(&pr, ordinal) == cudaSuccess) {
-      const unsigned char* b = (const unsigned char*)pr.uuid.bytes;
-      snprintf(uuid, sizeof uuid, "GPU-%02x%02x%02x%02x-%02x%02x-%02x%02x-%02x%02x-%02x%02x%02x%02x%02x%02x", b[0], b[1], b[2], b[3], b[4], b[5], b[6], b[7],
-               b[8], b[9], b[10], b[11], b[12], b[13], b[14], b[15]);
-    } else {
-      cudaGetLastError();
-    }
+  try {
+    device_identity(ordinal, bus, sizeof bus, uuid, sizeof uuid);
+  } catch (const Error&) {  // the manifest says "unknown" with empty strings
+    cudaGetLastError();
+    bus[0] = uuid[0] = 0;
   }
   o << "{\"apiVersion\":\"kukeon.gpupool/v1\",\"kind\":\"PoolManifest\",\"device\":" << ordinal << ",\"deviceUUID\":\"" << uuid << "\",\"pciBusId\":\"" << bus
-    << "\",\"poolBytes\":" << m->pool_bytes[(size_t)li] << ",\"mode\":" << m->plan.mode << ",\"format\":\"" << m->plan.index.format
+    << "\",\"poolBytes\":" << m->pools[(size_t)li].bytes << ",\"mode\":" << m->plan.mode << ",\"format\":\"" << m->plan.index.format
     << "\",\"align\":" << KK_POOL_ALIGN << ",\"tensors\":[";
   for (size_t i = 0; i < T.size(); ++i) {
     const DtypeInfo* di = dtype_info(pl[i].dtype);
@@ -1218,32 +1137,31 @@ std::string model_stats(kk_model* m) {
 // ---------------------------------------------------------------------------------------------
 void model_stage_resident(kk_model* m) {
   std::lock_guard<std::mutex> op(m->op_mu);
-  if (!is_raw(m)) free_resident(m);
-  else if (m->raw.empty()) fail(KK_ESTATE, "the raw image of this model has been released");
+  if (!is_raw(m)) m->images.clear();
+  else if (m->images.empty()) fail(KK_ESTATE, "the raw image of this model has been released");
   FdSet fds(m->plan.index.shards, map_policy());
   if (is_raw(m)) {  // RAW: the resident image IS the raw image; stage this process's own part(s), no fan-out
-    for (size_t li = 0; li < m->dev_idx.size(); ++li) stage_image(m, (int)li, m->local_parts[li], fds, m->raw[li].image, m->img_off[(size_t)m->local_parts[li]]);
+    for (size_t li = 0; li < m->dev_idx.size(); ++li)
+      stage_image(m, (int)li, m->local_parts[li], fds, m->images[li].image.get(), m->img_off[(size_t)m->local_parts[li]]);
     return;
   }
-  m->resident.resize(m->dev_idx.size());
+  std::vector<DeviceImage> images(m->dev_idx.size());
   for (size_t li = 0; li < m->dev_idx.size(); ++li) {
-    Device& dev = m->ctx->devs[(size_t)m->dev_idx[li]];
-    KK_CUDA(cudaSetDevice(dev.ordinal));
+    const int ordinal = m->ctx->devs[(size_t)m->dev_idx[li]].ordinal;
     const ImageLayout im = lay_out_image(m->plan, {m->local_parts[li]});
-    auto& R = m->resident[li];
-    const uint64_t bytes = im.bytes ? im.bytes : 256;
-    cudaError_t e = cudaMalloc((void**)&R.image, bytes);
-    if (e != cudaSuccess) { cudaGetLastError(); R.image = nullptr; fail(KK_ENOMEM, "device %d: cudaMalloc(%llu) for the resident image failed", dev.ordinal, (unsigned long long)bytes); }
-    stage_image(m, (int)li, m->local_parts[li], fds, R.image, im.chunk_off[0]);
-    R.d_segs = upload_segs(im.segs);
+    DeviceImage& R = images[li];
+    R.image = DevBuf(ordinal, im.bytes ? im.bytes : 256, "the resident image");
+    stage_image(m, (int)li, m->local_parts[li], fds, R.image.get(), im.chunk_off[0]);
+    R.segs = upload_segs(ordinal, im.segs);
     R.launches = im.launches;
   }
+  m->images = std::move(images);
 }
 
 void model_unstage_resident(kk_model* m) {
   std::lock_guard<std::mutex> op(m->op_mu);
   if (is_raw(m)) return;  // the raw image lives as long as a deferred RAW model does
-  free_resident(m);
+  m->images.clear();
 }
 
 // RAW: the stage-1 fan-out alone (own part of the image -> every peer image), one launch per local device.  Otherwise the resident image's
@@ -1252,16 +1170,16 @@ void model_convert_resident(kk_model* m, float* ms_total, float* ms_per_launch, 
   std::lock_guard<std::mutex> op(m->op_mu);
   const size_t nl = m->dev_idx.size();
   std::vector<std::vector<ConvertLaunch>> launches(nl);
-  std::vector<DevScratch> tables(nl);  // RAW: the fan-out launches' segment tables
+  std::vector<DevBuf> tables(nl);  // RAW: the fan-out launches' segment tables
   if (is_raw(m)) {
-    if (m->raw.empty()) fail(KK_ESTATE, "the raw image of this model has been released");
+    if (m->images.empty()) fail(KK_ESTATE, "the raw image of this model has been released");
     for (size_t li = 0; li < nl; ++li) raw_fanout_launch(m, (int)li, tables[li], launches[li]);
   } else {
-    if (m->resident.size() != nl) fail(KK_ESTATE, "kk_stage_resident has not been called");
+    if (m->images.size() != nl) fail(KK_ESTATE, "kk_stage_resident has not been called");
     for (size_t li = 0; li < nl; ++li) {
       ConvertLaunch base{};
       fill_dsts(m, (int)li, base);
-      launches[li] = image_launches(base, m->resident[li].image, m->resident[li].d_segs, m->resident[li].launches);
+      launches[li] = image_launches(base, m->images[li]);
     }
   }
   std::vector<float> per;

@@ -12,27 +12,41 @@
 
 #include "kk_common.hpp"
 #include "kk_kernels.cuh"
-#include "kk_nvls.hpp"
+#include "kk_mem.hpp"
 #include "kk_plan.hpp"
-#include "kk_vmm.hpp"
 
 namespace kk {
 
-#define KK_CUDA(expr)                                                                               \
-  do {                                                                                              \
-    cudaError_t _e = (expr);                                                                        \
-    if (_e != cudaSuccess) ::kk::fail(KK_ECUDA, "%s: %s (%s)", #expr, cudaGetErrorString(_e), cudaGetErrorName(_e)); \
-  } while (0)
+// CUDA events that must not leak when a KK_CUDA check throws half way through a function.
+struct EventSet {
+  std::vector<cudaEvent_t> ev;
+  explicit EventSet(size_t n = 0) : ev(n, nullptr) {}
+  cudaEvent_t& operator[](size_t i) { return ev[i]; }
+  size_t size() const { return ev.size(); }
+  void create_all() {
+    for (auto& e : ev) KK_CUDA(cudaEventCreate(&e));
+  }
+  ~EventSet() {
+    for (auto e : ev)
+      if (e) cudaEventDestroy(e);
+  }
+  EventSet(const EventSet&) = delete;
+  EventSet& operator=(const EventSet&) = delete;
+  EventSet(EventSet&& o) noexcept : ev(std::move(o.ev)) { o.ev.clear(); }
+};
+
+// PCI bus id (lower case, as /proc/driver/nvidia/gpus/ names it) and UUID ("GPU-…") of a CUDA device; a null output is skipped.  Throws KK_ECUDA.
+void device_identity(int ordinal, char* bus, size_t bus_cap, char* uuid, size_t uuid_cap);
 
 struct Slot {
   uint8_t* pinned = nullptr;  // cudaHostAlloc'd, also mapped into the device address space
-  uint8_t* dev = nullptr;     // device staging buffer of the same size
+  DevBuf dev;                 // device staging buffer of the same size
   cudaEvent_t done = nullptr; // recorded after the convert kernel that consumed this slot
 };
 
 struct Reader {
   cudaStream_t stream = nullptr;
-  uint32_t* sched = nullptr;  // two zeroed device words: the tile-scheduling counters every launch on `stream` needs (ConvertLaunch::sched)
+  DevBuf sched;  // two zeroed device words: the tile-scheduling counters every launch on `stream` needs (ConvertLaunch::sched)
   std::vector<Slot> slots;
 };
 
@@ -44,7 +58,7 @@ struct Device {
   int sm_count = 0;
   std::vector<Reader> readers;
   cudaStream_t stream = nullptr;  // resident launches, checksum, misc
-  uint32_t* sched = nullptr;      // tile-scheduling counters every launch on `stream` needs (first 8 of 256 zeroed bytes)
+  DevBuf sched;                   // tile-scheduling counters every launch on `stream` needs (first 8 of 256 zeroed bytes)
   std::unique_ptr<std::mutex> sum_mu{new std::mutex};  // kk_checksum's accumulator is the 8 bytes at sched + 32 words: no cudaMalloc / cudaFree per call
   uint64_t pool_in_use = 0;
   bool kernels_ready = false;
@@ -62,6 +76,30 @@ struct PeerBuf {
 // One convert launch over a device image: its slice of the image's rebased segment table.
 struct ImageLaunch {
   uint32_t seg_begin, n_segs, n_tiles;
+};
+
+// Chunk buffers of plan parts staged back to back in HBM (lay_out_image): the resident image of kk_stage_resident, and the raw image of a
+// KK_FANOUT_RAW load, into which the file bytes of every part are all-gathered (stage 1) before every device converts all of it (stage 2).
+struct DeviceImage {
+  DevBuf image;
+  DevBuf segs;      // every part's segments rebased onto the image
+  std::vector<ImageLaunch> launches;
+  DevBuf copy_segs;  // RAW: one COPY segment per chunk of every part, [kk_model::chunk_base[part] + ci]
+};
+
+// The pool of one local device: cudaMalloc memory in whole 2 MiB multiples, a VMM allocation, or an alias into kk_model::nvls.  Its plan
+// bytes are reserved on Device::pool_in_use, and returned under kk_ctx::mu once the memory is gone.
+struct Pool {
+  uint8_t* ptr = nullptr;
+  uint64_t bytes = 0;             // plan bytes
+  DevBuf mem;                     // cudaMalloc backing
+  std::unique_ptr<VmmAlloc> vmm;  // KK_CFG_VMM_POOLS backing
+  kk_ctx* ctx = nullptr;          // set once `bytes` are reserved on dev->pool_in_use
+  Device* dev = nullptr;
+  bool is_nvls() const { return ptr && !mem && !vmm; }
+  Pool() = default;
+  Pool(const Pool&) = delete;
+  ~Pool();
 };
 
 }  // namespace kk
@@ -84,46 +122,29 @@ struct kk_model {
   // local devices that hold a pool, as indices into ctx->devs; local_parts[i] is the plan part device i ingests
   std::vector<int> dev_idx;
   std::vector<int> local_parts;
-  std::vector<uint8_t*> pools;       // per local device
-  std::vector<uint64_t> pool_bytes;  // per local device
+  // KK_FANOUT_NVLS (one process, >= 2 devices): per-device VMM allocations bound to one multicast object; the pools alias them, and this is
+  // declared before the pools so that it outlives them
+  std::unique_ptr<kk::NvlsPools> nvls;
+  std::vector<kk::Pool> pools;  // per local device
   // What kk_export hands out is fixed once the pools exist: the manifest text and the pool's CUDA IPC handle are built on first use and kept.  Every
   // cell that mounts the model exports again, and the calls underneath (cudaIpcGetMemHandle, cudaGetDeviceProperties) go through the driver's
   // system-wide lock, where they wait behind whatever another process on the host is doing in the driver.
   std::mutex export_mu;
   std::vector<std::string> manifest_cache;               // per local device, empty = not built yet
   std::vector<std::vector<uint8_t>> pool_handle_cache;   // per local device, empty = not asked yet
-  std::vector<KKSeg*> d_segs;        // per local device: device copy of its part's segment table
+  std::vector<kk::DevBuf> d_segs;    // per local device: device copy of its part's segment table
   kk::PeerBuf peer[kk::kPeerKinds][KK_MAX_DEVICES];  // [kind][rank]
-  // resident image (kernel-stage measurement)
-  struct Resident {
-    uint8_t* image = nullptr;
-    KKSeg* d_segs = nullptr;
-    std::vector<kk::ImageLaunch> launches;
-  };
-  std::vector<Resident> resident;  // per local device
-  // KK_FANOUT_RAW: the file bytes of every part are all-gathered into a per-device raw image (stage 1, fan-out of
-  // the *quantised* bytes), then every device converts the whole image into its own pool (stage 2).
-  struct Raw {
-    uint8_t* image = nullptr;
-    uint64_t bytes = 0;
-    KKSeg* d_copy_segs = nullptr;  // one COPY segment per chunk of every part: [chunk_base[part] + ci]
-    KKSeg* d_conv_segs = nullptr;  // every part's segments rebased onto the image
-    std::vector<kk::ImageLaunch> conv_launches;
-  };
-  std::vector<Raw> raw;                         // per local device (empty unless fanout == RAW)
+  // Per local device.  KK_FANOUT_RAW: the raw image (the resident image too), allocated with the pools; empty once released.  Otherwise the
+  // resident image (kernel-stage measurement), staged by kk_stage_resident.
+  std::vector<kk::DeviceImage> images;
   std::vector<std::vector<uint64_t>> img_off;   // [part][chunk] offset of the chunk buffer inside the raw image
   std::vector<uint32_t> chunk_base;             // prefix sum of chunk counts per part
   // KK_FANOUT_PULL (one process per GPU): this rank's part of the pool, [slice_lo, slice_hi), also lives in slice_buf (a separate,
   // small allocation — the only thing peers have to map); slice_buf[0] corresponds to pool offset slice_base
-  uint8_t* slice_buf = nullptr;
+  kk::DevBuf slice_buf;
   uint64_t slice_base = 0;
   std::vector<std::pair<uint64_t, uint64_t>> part_range;  // [lo, hi) pool bytes every part produces
   bool raw_staged = false;                      // stage 1 complete on this process since the last conversion
-  // KK_FANOUT_NVLS (one process, >= 2 devices): the pools are VMM allocations bound to one multicast object; pools[i] then
-  // aliases nvls->pool(i) and must not be cudaFree'd
-  std::unique_ptr<kk::NvlsPools> nvls;
-  // KK_CFG_VMM_POOLS: pools[i] aliases vmm[i]->ptr() (cuMemCreate memory, exportable as a POSIX fd and mappable read-only elsewhere); never cudaFree'd
-  std::vector<std::unique_ptr<kk::VmmAlloc>> vmm;
   // state
   std::mutex op_mu;  // serialises the data-moving calls on ONE model (kk_load_part, kk_convert_local, kk_*_resident) against each other
   std::mutex peer_mu;  // guards peer[]; slice attach takes only this lock: stage 1 of a PULL load never reads the slice table, so slice buffers may be attached WHILE kk_load_part runs

@@ -16,8 +16,9 @@ from tests.test_gpu_load import assert_pool_matches
 pytestmark = pytest.mark.gpu
 MB = 1 << 20
 
-_CHILD = r'''
-import json, sys
+# The consumer: receives the pool's fd over the staged socket and finds the exporter's GPU by its UUID.
+_CHILD_SETUP = r'''
+import json, os, sys
 import numpy as np
 sys.path.insert(0, sys.argv[1])
 from kukeon_b200 import gpupool, modelhub
@@ -32,6 +33,9 @@ for i in range(cnt):
     if "GPU-%s-%s-%s-%s-%s" % (b[0:4].hex(), b[4:6].hex(), b[6:8].hex(), b[8:10].hex(), b[10:16].hex()) == want_uuid: dev = i
 assert dev is not None
 out = {}
+'''
+
+_CHILD = _CHILD_SETUP + r'''
 im = gpupool.ImportedPool(fd, dev, size, readonly=True)
 buf = np.empty(n, np.uint8)
 err, = cudart.cudaMemcpy(buf.ctypes.data, im.ptr + off, n, cudart.cudaMemcpyKind.cudaMemcpyDeviceToHost); assert err == 0, err
@@ -42,8 +46,22 @@ e2, = cudart.cudaDeviceSynchronize()
 out["write_errors"] = [int(e1), int(e2)]
 print(json.dumps(out))
 sys.stdout.flush()
-import os
 os._exit(0)  # the context may be poisoned by the fault: do not run teardown through it
+'''
+
+# Reads only: maps the pool read-only twice, each time reading the bytes back and closing the import (kk_import_close unmaps and releases
+# the mapping; the second import finds nothing of the first left over), then exits through the normal teardown.
+_CHILD_READ = _CHILD_SETUP + r'''
+out["hex"] = []
+for _ in range(2):
+    im = gpupool.ImportedPool(fd, dev, size, readonly=True)
+    buf = np.empty(n, np.uint8)
+    err, = cudart.cudaMemcpy(buf.ctypes.data, im.ptr + off, n, cudart.cudaMemcpyKind.cudaMemcpyDeviceToHost); assert err == 0, err
+    out["hex"].append(buf.tobytes().hex())
+    im.close()
+os.close(fd)
+err, = cudart.cudaDeviceSynchronize(); assert err == 0, err
+print(json.dumps(out))
 '''
 
 
@@ -123,3 +141,31 @@ def test_ipc_mount_detects_a_pool_that_was_written_to(pool, tmp_path):
     finally:
         modelhub.forget_pool(m)
         m.release()
+
+
+def test_another_process_reads_the_pool_through_a_read_only_import_and_closes_it(native, tmp_path):
+    p = str(tmp_path / "m.safetensors")
+    helpers.mixed_safetensors(p)
+    shards, recs = oracle.index_path(p)
+    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    with gpupool.Pool([0], n_staging_buffers=2, staging_buffer_bytes=4 * MB, n_reader_threads=1, flags=gpupool.CFG_VMM_POOLS) as pl:
+        m = pl.load(p)
+        spec = None
+        try:
+            spec = modelhub.Mount(m, 0, str(tmp_path / "cell" / "container"))
+            env = dict(e.split("=", 1) for e in spec.env)
+            want, _ = oracle.plan_pool(recs)
+            t = want[7]  # h.bf16.big
+            exp, _ = oracle.expected_pool(shards, recs)
+            before = m.checksum(0, 0, m.info()["pool_bytes"] // 8 * 8)
+            r = subprocess.run([sys.executable, "-c", _CHILD_READ, root, os.path.join(spec.host_dir, "pool.sock"), str(t["pool_offset"]), "4096",
+                                env["KUKEON_GPUPOOL_DEVICE_UUID"]], capture_output=True, text=True, timeout=180)
+            assert r.returncode == 0, r.stderr[-2000:]
+            out = json.loads(r.stdout.strip().splitlines()[-1])
+            assert [bytes.fromhex(h) for h in out["hex"]] == [exp[t["pool_offset"]:t["pool_offset"] + 4096].tobytes()] * 2
+            assert m.checksum(0, 0, m.info()["pool_bytes"] // 8 * 8) == before
+            assert_pool_matches(m, 0, shards, recs)
+        finally:
+            if spec is not None:
+                modelhub.unmount(spec)
+            m.release()
