@@ -238,8 +238,8 @@ int kk_model_get_info(kk_model* m, kk_model_info* o) {
     uint64_t pb = 0;
     for (auto& pool : m->pools) pb = pool.bytes > pb ? pool.bytes : pb;
     o->pool_bytes = pb;
-    o->n_devices = (int32_t)m->dev_idx.size();
-    for (size_t i = 0; i < m->dev_idx.size(); ++i) o->devices[i] = m->ctx->devs[(size_t)m->dev_idx[i]].ordinal;
+    o->n_devices = (int32_t)m->pools.size();
+    for (size_t i = 0; i < m->pools.size(); ++i) o->devices[i] = m->ctx->devs[i].ordinal;
     o->mode = m->plan.mode;
     {
       std::lock_guard<std::mutex> g(m->ctx->mu);
@@ -267,15 +267,15 @@ int kk_placements(kk_model* m, const char* tensor, kk_placement* out, size_t cap
     for (size_t i = 0; i < T.size(); ++i)
       if (T[i].name == tensor) { ti = i; break; }
     if (ti == T.size()) kk::fail(KK_ENOENT, "tensor \"%s\" not in this model", tensor);
-    const size_t nl = m->dev_idx.size();
+    const size_t nl = m->pools.size();
     if (n) *n = nl;
     if (!out) return;
     if (cap < nl) kk::fail(KK_ERANGE, "need room for %zu placements", nl);
     for (size_t li = 0; li < nl; ++li) {
-      const kk::Placement& p = m->plan.placement_of_part(m->local_parts[li])[ti];
+      const kk::Placement& p = m->plan.placement_of_part(m->shape.local_parts[li])[ti];
       kk_placement& o = out[li];
       memset(&o, 0, sizeof o);
-      o.device = m->ctx->devs[(size_t)m->dev_idx[li]].ordinal;
+      o.device = m->ctx->devs[li].ordinal;
       o.dtype = p.dtype;
       o.pool_offset = p.pool_offset;
       o.nbytes = p.nbytes;
@@ -408,7 +408,7 @@ int kk_checksum(kk_model* m, int device, uint64_t off, uint64_t nbytes, uint64_t
     const kk::Pool& pool = m->pools[(size_t)li];
     if (off > pool.bytes || nbytes > pool.bytes - off) kk::fail(KK_EINVAL, "range outside the pool");
     if (off % 8) kk::fail(KK_EINVAL, "pool_offset must be a multiple of 8");
-    kk::Device& d = m->ctx->devs[(size_t)m->dev_idx[(size_t)li]];
+    kk::Device& d = m->ctx->devs[(size_t)li];
     KK_CUDA(cudaSetDevice(device));
     // the accumulator lives in the device's scratch words: a cudaMalloc + cudaFree pair per call synchronises the whole device and, next to a
     // 16 GB pool, stalls for tens of milliseconds every few calls

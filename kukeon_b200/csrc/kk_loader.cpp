@@ -152,8 +152,6 @@ void pad_dsts_for_test(ConvertLaunch& L) {
   while (L.n_dst < (uint32_t)want && L.n_dst < KK_MAX_DST) { L.dst[L.n_dst] = L.dst[L.n_dst % have]; L.n_dst++; }
 }
 
-bool is_nvls(const kk_model* m) { return m->opts.fanout == KK_FANOUT_NVLS && m->plan.mode == KK_MODE_BROADCAST && m->nvls; }
-
 // multimem.st exists for 4-, 8- and 16-byte accesses only: a plan qualifies for KK_LAUNCH_MULTIMEM when no segment ever needs a 1- or
 // 2-byte store — every tile of it is whole 16-byte output vectors.  Transposes store single elements at tile edges and are excluded; FP8
 // widening works on 16-element groups and needs whole groups.
@@ -169,65 +167,65 @@ bool plan_allows_multimem(const Plan& P, std::string* why) {
   return true;
 }
 
-bool is_pull(const kk_model* m) { return m->opts.fanout == KK_FANOUT_PULL && m->plan.mode == KK_MODE_BROADCAST; }
-bool is_raw(const kk_model* m) { return m->opts.fanout == KK_FANOUT_RAW && m->plan.mode == KK_MODE_BROADCAST; }
-
-// Pool bytes [lo, hi) that plan part `part` produces.  Pool order equals file order, so for every op that writes its output
-// linearly this is one contiguous range and the ranges of different parts are disjoint.  Returns false when the part carries ops
-// whose output is not linear in the pool (the scatter row exchange; transposes, whose strided stores interleave with the other parts'
-// inside the tensor-wide extent stats() reports for them): such plans cannot be pulled slice by slice.
+// Pool bytes [lo, hi) that plan part `part` produces, KK_OP_ROWSPLIT segments left out (their rows land in every rank's pool).  Pool
+// order equals file order, so for every op that writes its output linearly this is one contiguous range and the ranges of different
+// parts are disjoint.  Returns false when the part carries ops whose output is not linear in the pool (the scatter row exchange;
+// transposes, whose strided stores interleave with the other parts' inside the tensor-wide extent counted here): such plans cannot be
+// pulled slice by slice.
 bool part_pool_range(const Plan& P, int part, uint64_t& lo, uint64_t& hi) {
   lo = UINT64_MAX;
   hi = 0;
+  bool linear = true;
   for (auto& s : P.parts[(size_t)part].segs) {
-    if (kk_is_transpose(s.op) || s.op == KK_OP_ROWSPLIT) return false;
+    if (s.op == KK_OP_ROWSPLIT) { linear = false; continue; }
+    if (kk_is_transpose(s.op)) linear = false;
     lo = std::min(lo, s.dst_off);
     hi = std::max(hi, s.dst_off + seg_out_extent(s));
   }
-  if (lo == UINT64_MAX) lo = hi = 0;
-  return true;
+  if (lo == UINT64_MAX) lo = 0;
+  return linear;
 }
 
 // Destination pools a convert launch on local device `li` writes to.
 void fill_dsts(kk_model* m, int li, ConvertLaunch& L) {
+  const LoadShape& S = m->shape;
   L.n_dst = 0;
   L.flags = 0;
   for (auto& d : L.dst) d = nullptr;
   L.dst[L.n_dst++] = m->pools[(size_t)li].ptr;
   L.n_xdst = 0;
   for (auto& d : L.xdst) d = nullptr;
-  if (m->plan.mode == KK_MODE_SCATTER && (m->plan.flags & KK_LOAD_SCATTER_EXCHANGE) && m->plan.n_parts > 1) {
+  if (S.xdst) {
     // all-to-all destinations of KK_OP_ROWSPLIT segments: the pool of every rank, indexed by rank
-    const int n = m->plan.n_parts;
-    for (int j = 0; j < n; ++j) {
+    for (int j = 0; j < S.n_parts; ++j) {
       uint8_t* p = nullptr;
-      if (m->opts.part_count > 1) p = (j == m->opts.part_index) ? m->pools[0].ptr : (uint8_t*)m->peer[kPeerPool][j].ptr;
-      else if (m->ctx->peer_ok) p = m->pools[(size_t)j].ptr;
+      if (S.multi_proc) p = (j == S.rank) ? m->pools[0].ptr : (uint8_t*)m->peer[kPeerPool][j].ptr;
+      else if (S.peer_ok) p = m->pools[(size_t)j].ptr;
       if (!p) fail(KK_ESTATE, "KK_LOAD_SCATTER_EXCHANGE: the pool of rank %d is not reachable (attach it with kk_peer_attach, or enable peer access)", j);
       L.xdst[j] = p;
     }
-    L.n_xdst = (uint32_t)n;
+    L.n_xdst = (uint32_t)S.n_parts;
   }
-  if (is_nvls(m)) {  // one multimem.st per vector reaches every pool through the switch
-    L.dst[0] = m->nvls->multicast();
-    L.n_dst = 1;
-    L.flags |= KK_LAUNCH_MULTIMEM;
-    return;
-  }
-  if (is_pull(m)) {  // stage 1 of a pull load: the same bytes into the slice buffer the peers will read (pool offset -> slice_buf - slice_base)
-    if (m->slice_buf) L.dst[L.n_dst++] = (uint8_t*)((uintptr_t)m->slice_buf.get() - (uintptr_t)m->slice_base);
-    return;
-  }
-  if (m->plan.mode != KK_MODE_BROADCAST || m->opts.fanout == KK_FANOUT_NONE) {
-    pad_dsts_for_test(L);
-    return;
-  }
-  if (m->opts.part_count > 1) {
-    for (auto& b : m->peer[kPeerPool])
-      if (b.ptr) L.dst[L.n_dst++] = (uint8_t*)b.ptr;
-  } else if (m->ctx->peer_ok) {
-    for (size_t j = 0; j < m->pools.size(); ++j)
-      if ((int)j != li) L.dst[L.n_dst++] = m->pools[j].ptr;
+  switch (S.order) {
+    case LoadOrder::kNvls:  // one multimem.st per vector reaches every pool through the switch
+      L.dst[0] = m->nvls->multicast();
+      L.n_dst = 1;
+      L.flags |= KK_LAUNCH_MULTIMEM;
+      return;
+    case LoadOrder::kPull:  // stage 1 of a pull load: the same bytes into the slice buffer the peers will read (pool offset -> slice_buf - slice_base)
+      if (m->slice_buf) L.dst[L.n_dst++] = (uint8_t*)((uintptr_t)m->slice_buf.get() - (uintptr_t)m->slice_base);
+      return;
+    case LoadOrder::kPush:
+      if (S.multi_proc) {
+        for (auto& b : m->peer[kPeerPool])
+          if (b.ptr) L.dst[L.n_dst++] = (uint8_t*)b.ptr;
+      } else {
+        for (size_t j = 0; j < m->pools.size(); ++j)
+          if ((int)j != li) L.dst[L.n_dst++] = m->pools[j].ptr;
+      }
+      break;
+    default:  // the own pool alone (a RAW model converts through convert_local_all)
+      break;
   }
   pad_dsts_for_test(L);
 }
@@ -237,7 +235,7 @@ void fill_raw_dsts(kk_model* m, int li, ConvertLaunch& L) {
   L.n_dst = 0;
   L.flags = 0;
   for (auto& d : L.dst) d = nullptr;
-  if (m->opts.part_count > 1) {
+  if (m->shape.multi_proc) {
     for (auto& b : m->peer[kPeerRaw])
       if (b.ptr) L.dst[L.n_dst++] = (uint8_t*)b.ptr;
   } else {
@@ -253,7 +251,7 @@ void fill_raw_dsts(kk_model* m, int li, ConvertLaunch& L) {
 template <class Consume>
 void stream_part(kk_model* m, int li, int part, const FdSet& fds, bool record_times, const Consume& consume) {
   kk_ctx* c = m->ctx;
-  Device& dev = c->devs[(size_t)m->dev_idx[(size_t)li]];
+  Device& dev = c->devs[(size_t)li];
   const PartPlan& pp = m->plan.parts[(size_t)part];
   std::lock_guard<std::mutex> pipeline(*dev.load_mu);
   std::atomic<size_t> next{0};
@@ -309,7 +307,7 @@ void stream_part(kk_model* m, int li, int part, const FdSet& fds, bool record_ti
 void convert_part(kk_model* m, int li, int part, const FdSet& fds) {
   const PartPlan& pp = m->plan.parts[(size_t)part];
   if (pp.chunks.empty()) return;
-  const int sm_count = m->ctx->devs[(size_t)m->dev_idx[(size_t)li]].sm_count;
+  const int sm_count = m->ctx->devs[(size_t)li].sm_count;
   const bool zerocopy = (m->ctx->cfg.flags & KK_CFG_ZEROCOPY) != 0;
   const KKSeg* d_segs = m->d_segs[(size_t)li].get<KKSeg>() + seg_base_of(m->plan, part);
   ConvertLaunch base{};
@@ -333,14 +331,14 @@ void convert_part(kk_model* m, int li, int part, const FdSet& fds) {
 // Stage 1 of a RAW load on local device li: file bytes of its plan part -> local raw image (H2D straight into place) -> peers' raw images
 // (COPY launch per chunk, bulk TMA stores over NVLink).
 void raw_stage1(kk_model* m, int li, const FdSet& fds) {
-  const int part = m->local_parts[(size_t)li];
+  const int part = m->shape.local_parts[(size_t)li];
   const PartPlan& pp = m->plan.parts[(size_t)part];
   if (pp.chunks.empty()) return;
-  const int sm_count = m->ctx->devs[(size_t)m->dev_idx[(size_t)li]].sm_count;
+  const int sm_count = m->ctx->devs[(size_t)li].sm_count;
   const DeviceImage& R = m->images[(size_t)li];
   ConvertLaunch base{};
   fill_raw_dsts(m, li, base);
-  if (base.n_dst > 0 && !m->ctx->peer_ok && m->opts.part_count <= 1) fail(KK_EUNSUPPORTED, "KK_FANOUT_RAW needs peer access between the context's devices");
+  if (base.n_dst > 0 && !m->shape.multi_proc && !m->shape.peer_ok) fail(KK_EUNSUPPORTED, "KK_FANOUT_RAW needs peer access between the context's devices");
   stream_part(m, li, part, fds, true, [&](Reader& rd, Slot& s, size_t ci) {
     const Chunk& ch = pp.chunks[ci];
     KK_CUDA(cudaMemcpyAsync(R.image.get() + m->img_off[(size_t)part][ci], s.pinned, ch.buf_bytes, cudaMemcpyHostToDevice, rd.stream));
@@ -363,7 +361,8 @@ void stage_image(kk_model* m, int li, int part, const FdSet& fds, uint8_t* image
   });
 }
 
-// Allocate the raw images and build the stage-1 (copy) and stage-2 (convert) segment tables.
+// Allocate the raw images and build their segment tables: stage 1's copies (one launch per chunk), the fan-out launch's copies and
+// stage 2's conversions.
 void setup_raw(kk_model* m) {
   const Plan& P = m->plan;
   std::vector<int> all;
@@ -372,6 +371,8 @@ void setup_raw(kk_model* m) {
   m->img_off = im.chunk_off;
   m->chunk_base.assign(P.parts.size(), 0);
   std::vector<KKSeg> copy_segs;
+  std::vector<std::vector<KKSeg>> fanout_segs(P.parts.size());  // [part]: the same copies with tile_begin running over the part
+  std::vector<uint32_t> fanout_tiles(P.parts.size(), 0);
   for (size_t p = 0; p < P.parts.size(); ++p) {
     m->chunk_base[p] = (uint32_t)copy_segs.size();
     for (size_t ci = 0; ci < P.parts[p].chunks.size(); ++ci) {
@@ -380,15 +381,21 @@ void setup_raw(kk_model* m) {
       cs.units = align_up(P.parts[p].chunks[ci].buf_bytes, 16);
       cs.op = KK_OP_COPY;
       copy_segs.push_back(cs);
+      cs.tile_begin = fanout_tiles[p];
+      fanout_tiles[p] += (uint32_t)kk_seg_tiles(KK_OP_COPY, cs.units, 0);
+      fanout_segs[p].push_back(cs);
     }
   }
-  m->images.resize(m->dev_idx.size());
-  for (size_t li = 0; li < m->dev_idx.size(); ++li) {
-    const int ordinal = m->ctx->devs[(size_t)m->dev_idx[li]].ordinal;
+  m->images.resize(m->pools.size());
+  for (size_t li = 0; li < m->images.size(); ++li) {
+    const int ordinal = m->ctx->devs[li].ordinal;
+    const int part = m->shape.local_parts[li];
     DeviceImage& R = m->images[li];
     // 2 MiB multiples: cheap to map over CUDA IPC (see the slice buffer in model_load)
     R.image = DevBuf(ordinal, align_up(im.bytes ? im.bytes : 256, 2u << 20), "the raw image");
     R.copy_segs = upload_segs(ordinal, copy_segs);
+    R.fanout_segs = upload_segs(ordinal, fanout_segs[(size_t)part]);
+    R.fanout = {0, (uint32_t)fanout_segs[(size_t)part].size(), fanout_tiles[(size_t)part]};
     R.segs = upload_segs(ordinal, im.segs);
     R.launches = im.launches;
   }
@@ -415,7 +422,7 @@ float time_launches(kk_model* m, std::vector<std::vector<ConvertLaunch>>& launch
   evs.reserve(launches.size());
   size_t most = 0;
   for (size_t li = 0; li < launches.size(); ++li) {
-    Device& dev = m->ctx->devs[(size_t)m->dev_idx[li]];
+    Device& dev = m->ctx->devs[li];
     KK_CUDA(cudaSetDevice(dev.ordinal));
     evs.emplace_back(launches[li].size() + 1);
     evs[li].create_all();
@@ -430,8 +437,8 @@ float time_launches(kk_model* m, std::vector<std::vector<ConvertLaunch>>& launch
   float worst = 0.f;
   if (per_launch) per_launch->assign(most, 0.f);
   for (size_t li = 0; li < launches.size(); ++li) {
-    KK_CUDA(cudaSetDevice(m->ctx->devs[(size_t)m->dev_idx[li]].ordinal));
-    KK_CUDA(cudaStreamSynchronize(m->ctx->devs[(size_t)m->dev_idx[li]].stream));
+    KK_CUDA(cudaSetDevice(m->ctx->devs[li].ordinal));
+    KK_CUDA(cudaStreamSynchronize(m->ctx->devs[li].stream));
     const size_t n = launches[li].size();
     float ms = 0.f;
     KK_CUDA(cudaEventElapsedTime(&ms, evs[li][0], evs[li][n]));
@@ -446,7 +453,7 @@ float time_launches(kk_model* m, std::vector<std::vector<ConvertLaunch>>& launch
 
 // Stage 2: every local device converts the whole gathered image into its own pool.
 void convert_local_all(kk_model* m, float* ms_total) {
-  std::vector<std::vector<ConvertLaunch>> launches(m->dev_idx.size());
+  std::vector<std::vector<ConvertLaunch>> launches(m->pools.size());
   for (size_t li = 0; li < launches.size(); ++li) {
     ConvertLaunch base{};
     base.n_dst = 1;
@@ -460,7 +467,7 @@ void convert_local_all(kk_model* m, float* ms_total) {
 // Stage 2 of a KK_FANOUT_PULL load: one COPY launch whose segments read every attached peer's slice buffer over NVLink (bulk loads)
 // and write the local pool.  Segments start with the peer after this rank so that the N ranks do not all read GPU 0 first.
 void pull_slices(kk_model* m, float* ms_total) {
-  const int n = m->opts.part_count, me = m->opts.part_index;
+  const int n = m->shape.n_parts, me = m->shape.rank;
   const PeerBuf* slice = m->peer[kPeerSlice];
   std::vector<int> peers;
   std::lock_guard<std::mutex> peer_lock(m->peer_mu);
@@ -493,7 +500,7 @@ void pull_slices(kk_model* m, float* ms_total) {
       segs.push_back(sg);
     }
     if (tiles > 0xFFFFFFF0ull) fail(KK_EUNSUPPORTED, "too many tiles for one pull launch");
-    table = upload_segs(m->ctx->devs[(size_t)m->dev_idx[0]].ordinal, segs);
+    table = upload_segs(m->ctx->devs[0].ordinal, segs);
     ConvertLaunch L{};
     L.src = (const uint8_t*)base;
     L.segs = table.get<KKSeg>();
@@ -508,29 +515,17 @@ void pull_slices(kk_model* m, float* ms_total) {
 }
 
 // RAW, kernel-stage measurement: stage 1's fan-out without the file reads — one COPY launch over all of local device li's own chunks, from
-// its raw image into every peer image.  table receives the launch's segment table.
-void raw_fanout_launch(kk_model* m, int li, DevBuf& table, std::vector<ConvertLaunch>& out) {
+// its raw image into every peer image.
+void raw_fanout_launch(kk_model* m, int li, std::vector<ConvertLaunch>& out) {
   ConvertLaunch L{};
   fill_raw_dsts(m, li, L);
-  const int part = m->local_parts[(size_t)li];
-  const PartPlan& pp = m->plan.parts[(size_t)part];
-  if (L.n_dst == 0 || pp.chunks.empty()) return;
-  std::vector<KKSeg> segs(pp.chunks.size());
-  uint32_t tiles = 0;
-  for (size_t ci = 0; ci < pp.chunks.size(); ++ci) {
-    KKSeg& sg = segs[ci];
-    sg.src_off = sg.dst_off = m->img_off[(size_t)part][ci];
-    sg.units = align_up(pp.chunks[ci].buf_bytes, 16);
-    sg.op = KK_OP_COPY;
-    sg.tile_begin = tiles;
-    tiles += (uint32_t)kk_seg_tiles(KK_OP_COPY, sg.units, 0);
-  }
-  if (segs.size() > kMaxSegsPerLaunch) fail(KK_EUNSUPPORTED, "too many chunks for one raw fan-out launch");
-  table = upload_segs(m->ctx->devs[(size_t)m->dev_idx[(size_t)li]].ordinal, segs);
-  L.src = m->images[(size_t)li].image.get();
-  L.segs = table.get<KKSeg>();
-  L.n_segs = (uint32_t)segs.size();
-  L.n_tiles = tiles;
+  const DeviceImage& R = m->images[(size_t)li];
+  if (L.n_dst == 0 || R.fanout.n_segs == 0) return;
+  if (R.fanout.n_segs > kMaxSegsPerLaunch) fail(KK_EUNSUPPORTED, "too many chunks for one raw fan-out launch");
+  L.src = R.image.get();
+  L.segs = R.fanout_segs.get<KKSeg>();
+  L.n_segs = R.fanout.n_segs;
+  L.n_tiles = R.fanout.n_tiles;
   out.push_back(L);
 }
 
@@ -539,7 +534,7 @@ void close_peers(kk_model* m) {
   for (auto& kind : m->peer)
     for (PeerBuf& b : kind) {
       if (b.opened_by_ipc) {
-        cudaSetDevice(m->ctx->devs[(size_t)m->dev_idx[0]].ordinal);
+        cudaSetDevice(m->ctx->devs[0].ordinal);
         cudaIpcCloseMemHandle(b.ptr);
       }
       b = PeerBuf{};
@@ -714,24 +709,22 @@ void ctx_close(kk_ctx* c) {
 // model
 // ---------------------------------------------------------------------------------------------
 static void do_load(kk_model* m) {
+  const LoadShape& S = m->shape;
   const double t0 = now_s();
   FdSet fds(m->plan.index.shards, map_policy());
   m->t_files_open = now_s() - t0;
-  const size_t nl = m->dev_idx.size();
+  const size_t nl = m->pools.size();
   m->t_part.assign(nl, 0.0);
-  const bool multi_proc = m->opts.part_count > 1;
-  const bool replicas = !multi_proc && m->plan.mode == KK_MODE_BROADCAST && nl > 1 &&
-                        (m->opts.fanout == KK_FANOUT_NONE || !m->ctx->peer_ok);
   ErrorSink sink;
   auto per_dev = [&](int li) {
     try {
       const double a = now_s();
-      if (is_raw(m)) {
+      if (S.order == LoadOrder::kRaw) {
         raw_stage1(m, li, fds);
-      } else if (replicas) {
+      } else if (S.every_part) {
         for (int p = 0; p < m->plan.n_parts; ++p) convert_part(m, li, p, fds);
       } else {
-        convert_part(m, li, m->local_parts[(size_t)li], fds);
+        convert_part(m, li, S.local_parts[(size_t)li], fds);
       }
       m->t_part[(size_t)li] = now_s() - a;
     } catch (...) {
@@ -743,43 +736,25 @@ static void do_load(kk_model* m) {
   per_dev(0);
   for (auto& t : th) t.join();
   sink.rethrow();
-  if (is_raw(m)) {
-    m->raw_staged = true;
-    if (!multi_proc) {  // one process owns every device: all stage-1 work is done, convert now
-      convert_local_all(m, nullptr);
-      m->raw_staged = false;
-    }
-  }
+  if (S.order == LoadOrder::kRaw && !S.two_stage) convert_local_all(m, nullptr);  // one process owns every device: stage 1 is done everywhere
   const double tc = now_s();
   fds.cleanup();  // part of the load: unmapping a checkpoint-sized mapping is not free
   m->t_files_close = now_s() - tc;
   m->t_load = now_s() - t0;
   m->n_loads++;
+  std::lock_guard<std::mutex> g(m->ctx->mu);
+  if (!S.two_stage) m->loaded = true;  // a two-stage model is loaded once kk_convert_local has run
 }
 
 kk_model* model_load(kk_ctx* c, const std::string& path, const kk_load_opts& opts_in) {
   kk_load_opts opts = opts_in;
   if (opts.part_count <= 1) { opts.part_count = 1; opts.part_index = 0; }
-  if (opts.part_index < 0 || opts.part_index >= opts.part_count || opts.part_count > KK_MAX_DEVICES)
-    fail(KK_EINVAL, "part %d of %d out of range", opts.part_index, opts.part_count);
-  if (opts.mode < KK_MODE_SINGLE || opts.mode > KK_MODE_SCATTER) fail(KK_EINVAL, "unknown mode %d", opts.mode);
-  if (opts.fanout < KK_FANOUT_P2P || opts.fanout > KK_FANOUT_PULL) fail(KK_EINVAL, "unknown fanout %d", opts.fanout);
-  if (opts.fanout == KK_FANOUT_NVLS) {
-    // every "cannot do NVLS here" is KK_EUNSUPPORTED (the contract since the first ABI version), whatever the reason
-    if (opts.mode != KK_MODE_BROADCAST) fail(KK_EUNSUPPORTED, "fan-out NVLS only applies to KK_MODE_BROADCAST");
-    if (opts.part_count > 1) fail(KK_EUNSUPPORTED, "fan-out NVLS needs one process owning all devices (sharing a multicast object across processes is not implemented)");
-    if (c->cfg.n_devices < 2) fail(KK_EUNSUPPORTED, "fan-out NVLS needs at least two devices in the context");
+  LoadShape shape = resolve_load_shape(opts, c->cfg.n_devices, c->peer_ok);
+  if (shape.order == LoadOrder::kNvls) {
     std::vector<int> ords(c->cfg.devices, c->cfg.devices + c->cfg.n_devices);
     std::string why;
     if (!NvlsPools::supported(ords, &why)) fail(KK_EUNSUPPORTED, "fan-out NVLS: this host does not expose it: %s", why.c_str());
   }
-  if (opts.fanout == KK_FANOUT_RAW && opts.mode != KK_MODE_BROADCAST) fail(KK_EINVAL, "KK_FANOUT_RAW only applies to KK_MODE_BROADCAST");
-  const bool multi_proc = opts.part_count > 1;
-  if (opts.fanout == KK_FANOUT_PULL && opts.mode != KK_MODE_BROADCAST) fail(KK_EINVAL, "KK_FANOUT_PULL only applies to KK_MODE_BROADCAST");
-  if (opts.fanout == KK_FANOUT_PULL && !multi_proc)
-    fail(KK_EINVAL, "KK_FANOUT_PULL is for one-process-per-GPU operation (part_count > 1); one process owning the GPUs fans out with P2P stores");
-  if (multi_proc && c->cfg.n_devices != 1) fail(KK_EINVAL, "multi-process parts need a one-device context (got %d devices)", c->cfg.n_devices);
-  if (multi_proc && opts.mode == KK_MODE_SINGLE) fail(KK_EINVAL, "KK_MODE_SINGLE cannot be split into parts");
 
   std::ostringstream ks;
   ks << canon(path) << "|m" << opts.mode << "|f" << opts.fanout << "|x" << (opts.flags & ~KK_LOAD_DEFER) << "|p" << opts.part_index << "/" << opts.part_count;
@@ -798,46 +773,39 @@ kk_model* model_load(kk_ctx* c, const std::string& path, const kk_load_opts& opt
     m = new kk_model;
     m->ctx = c;
     m->key = key;
-    m->opts = opts;
+    m->shape = std::move(shape);
     m->refcount = 1;
     m->loading = true;
     c->models[key] = m;
   }
+  const LoadShape& S = m->shape;
   try {
     double t0 = now_s();
     Index ix = index_path(path);
     m->t_index = now_s() - t0;
     t0 = now_s();
-    int n_parts = 1;
-    if (opts.mode != KK_MODE_SINGLE) n_parts = multi_proc ? opts.part_count : c->cfg.n_devices;
-    int mode = opts.mode;
-    m->plan = build_plan(std::move(ix), mode, opts.flags & ~KK_LOAD_DEFER, n_parts, c->slot_bytes);
+    m->plan = build_plan(std::move(ix), opts.mode, opts.flags & ~KK_LOAD_DEFER, S.n_parts, c->slot_bytes);
     m->t_plan = now_s() - t0;
     t0 = now_s();
-    if (multi_proc || opts.mode == KK_MODE_SINGLE) {
-      m->dev_idx = {0};
-      m->local_parts = {multi_proc ? opts.part_index : 0};
-    } else {
-      for (int i = 0; i < c->cfg.n_devices; ++i) { m->dev_idx.push_back(i); m->local_parts.push_back(i); }
-    }
     // concatenated segment table of all parts
     std::vector<KKSeg> all;
     for (auto& pp : m->plan.parts) all.insert(all.end(), pp.segs.begin(), pp.segs.end());
-    m->pools = std::vector<Pool>(m->dev_idx.size());
-    m->d_segs.resize(m->dev_idx.size());
-    if (opts.fanout == KK_FANOUT_NVLS) {
+    const size_t nl = S.local_parts.size();
+    m->pools = std::vector<Pool>(nl);
+    m->d_segs.resize(nl);
+    if (S.order == LoadOrder::kNvls) {
       std::string why;
       if (!plan_allows_multimem(m->plan, &why)) fail(KK_EUNSUPPORTED, "fan-out NVLS: %s", why.c_str());
       std::vector<int> ords;
-      for (int di : m->dev_idx) ords.push_back(c->devs[(size_t)di].ordinal);
+      for (auto& d : c->devs) ords.push_back(d.ordinal);
       KK_CUDA(cudaSetDevice(ords[0]));  // the driver entry points below want a current context on the calling thread
       m->nvls.reset(new NvlsPools);
       m->nvls->create(ords, m->plan.pool_bytes_of_part(0));
     }
-    for (size_t li = 0; li < m->dev_idx.size(); ++li) {
-      Device& d = c->devs[(size_t)m->dev_idx[li]];
+    for (size_t li = 0; li < nl; ++li) {
+      Device& d = c->devs[li];
       KK_CUDA(cudaSetDevice(d.ordinal));
-      const uint64_t pb = m->plan.pool_bytes_of_part(m->local_parts[li]);
+      const uint64_t pb = m->plan.pool_bytes_of_part(S.local_parts[li]);
       Pool& pool = m->pools[li];
       {
         std::lock_guard<std::mutex> g(c->mu);
@@ -868,24 +836,23 @@ kk_model* model_load(kk_ctx* c, const std::string& path, const kk_load_opts& opt
       }
       m->d_segs[li] = upload_segs(d.ordinal, all);
     }
-    if (is_raw(m)) setup_raw(m);
-    if (is_pull(m)) {
+    if (S.order == LoadOrder::kRaw) setup_raw(m);
+    if (S.order == LoadOrder::kPull) {
       m->part_range.assign((size_t)m->plan.n_parts, {0, 0});
       for (int p = 0; p < m->plan.n_parts; ++p)
         if (!part_pool_range(m->plan, p, m->part_range[(size_t)p].first, m->part_range[(size_t)p].second))
           fail(KK_EUNSUPPORTED, "KK_FANOUT_PULL cannot be combined with transposing loads (their output is not one contiguous pool range per rank)");
-      const auto& mine = m->part_range[(size_t)opts.part_index];
+      const auto& mine = m->part_range[(size_t)S.rank];
       m->slice_base = mine.first & ~(uint64_t)255;
       const uint64_t sb = mine.second > m->slice_base ? mine.second - m->slice_base : 0;
       // whole 2 MiB multiples, like the pools: cudaIpcOpenMemHandle of such an allocation is far cheaper than of one the driver carved out of
       // shared blocks (at N = 8, seven rounded 16 GB pools map faster than seven 2 GB slice buffers of odd size)
-      m->slice_buf = DevBuf(c->devs[(size_t)m->dev_idx[0]].ordinal, align_up(sb ? sb : 256, 2u << 20), "the slice buffer");
+      m->slice_buf = DevBuf(c->devs[0].ordinal, align_up(sb ? sb : 256, 2u << 20), "the slice buffer");
     }
     m->t_alloc = now_s() - t0;
     if (!(opts.flags & KK_LOAD_DEFER)) {
       do_load(m);
-      m->loaded = !((is_raw(m) || is_pull(m)) && multi_proc);
-      if (is_raw(m) && !multi_proc) m->images.clear();  // the gathered file bytes are not needed once the pools are built
+      if (S.order == LoadOrder::kRaw && !S.two_stage) m->images.clear();  // the gathered file bytes are not needed once the pools are built
     }
   } catch (...) {
     {
@@ -906,43 +873,35 @@ kk_model* model_load(kk_ctx* c, const std::string& path, const kk_load_opts& opt
 
 void model_load_part(kk_model* m) {
   std::lock_guard<std::mutex> op(m->op_mu);
-  if (is_raw(m) && m->images.empty()) fail(KK_ESTATE, "the raw image of this model has been released");
+  if (m->shape.order == LoadOrder::kRaw && m->images.empty()) fail(KK_ESTATE, "the raw image of this model has been released");
   do_load(m);
-  std::lock_guard<std::mutex> g(m->ctx->mu);
-  if (!((is_raw(m) || is_pull(m)) && m->opts.part_count > 1)) m->loaded = true;  // multi-process RAW / PULL: loaded after kk_convert_local
 }
 
 void model_convert_local(kk_model* m, float* ms_total) {
   std::lock_guard<std::mutex> op(m->op_mu);
-  if (is_pull(m)) {
-    pull_slices(m, ms_total);
-    std::lock_guard<std::mutex> g(m->ctx->mu);
-    m->loaded = true;
-    return;
-  }
-  if (!is_raw(m) || m->images.empty()) fail(KK_ESTATE, "kk_convert_local only applies to KK_FANOUT_RAW models with a live raw image and to KK_FANOUT_PULL models");
-  convert_local_all(m, ms_total);
+  if (m->shape.order == LoadOrder::kPull) pull_slices(m, ms_total);
+  else if (m->shape.order == LoadOrder::kRaw && !m->images.empty()) convert_local_all(m, ms_total);
+  else fail(KK_ESTATE, "kk_convert_local only applies to KK_FANOUT_RAW models with a live raw image and to KK_FANOUT_PULL models");
   std::lock_guard<std::mutex> g(m->ctx->mu);
   m->loaded = true;
-  m->raw_staged = false;
 }
 
 void model_export_raw(kk_model* m, int li, void* handle_out) {
-  if (!is_raw(m) || m->images.empty()) fail(KK_ESTATE, "this model has no raw image");
-  KK_CUDA(cudaSetDevice(m->ctx->devs[(size_t)m->dev_idx[(size_t)li]].ordinal));
+  if (m->shape.order != LoadOrder::kRaw || m->images.empty()) fail(KK_ESTATE, "this model has no raw image");
+  KK_CUDA(cudaSetDevice(m->ctx->devs[(size_t)li].ordinal));
   cudaIpcMemHandle_t h;
   KK_CUDA(cudaIpcGetMemHandle(&h, m->images[(size_t)li].image.get()));
   memcpy(handle_out, &h, sizeof h);
 }
 
 void model_export_slice(kk_model* m, void* handle_out, bool as_pointer) {
-  if (!is_pull(m) || !m->slice_buf) fail(KK_ESTATE, "this model has no slice buffer (KK_FANOUT_PULL only)");
+  if (m->shape.order != LoadOrder::kPull || !m->slice_buf) fail(KK_ESTATE, "this model has no slice buffer (KK_FANOUT_PULL only)");
   if (as_pointer) {
     void* p = m->slice_buf.get();
     memcpy(handle_out, &p, sizeof p);
     return;
   }
-  KK_CUDA(cudaSetDevice(m->ctx->devs[(size_t)m->dev_idx[0]].ordinal));
+  KK_CUDA(cudaSetDevice(m->ctx->devs[0].ordinal));
   cudaIpcMemHandle_t h;
   KK_CUDA(cudaIpcGetMemHandle(&h, m->slice_buf.get()));
   memcpy(handle_out, &h, sizeof h);
@@ -971,7 +930,7 @@ void model_probe_peer(kk_model* m, int rank, PeerKind kind, uint64_t& nbytes, fl
   if (!src) fail(KK_ESTATE, "probe: rank %d has no attached buffer of that kind", rank);
   nbytes = std::min(nbytes, avail) & ~(uint64_t)255;
   if (!nbytes) fail(KK_EINVAL, "probe: nothing to copy from rank %d", rank);
-  Device& dev = m->ctx->devs[(size_t)m->dev_idx[0]];
+  Device& dev = m->ctx->devs[0];
   DevBuf tmp(dev.ordinal, nbytes, "the peer probe");
   EventSet ev(2);
   ev.create_all();
@@ -1001,18 +960,20 @@ void model_peer_attach(kk_model* m, PeerKind kind, int rank, const void* handle,
   // The mapping itself happens outside peer_mu (it is the slow part; several ranks may be attached concurrently), only the table update is locked.
   std::unique_lock<std::mutex> op(m->op_mu, std::defer_lock);
   if (kind != kPeerSlice) op.lock();
-  if (kind == kPeerRaw && !is_raw(m)) fail(KK_ESTATE, "raw peer attach needs a KK_FANOUT_RAW model");
-  if (kind == kPeerSlice && !is_pull(m)) fail(KK_ESTATE, "slice attach needs a KK_FANOUT_PULL model");
-  if (m->opts.part_count <= 1) fail(KK_ESTATE, "peer attach needs a multi-process (part_count > 1) model");
-  if (rank < 0 || rank >= m->opts.part_count || rank == m->opts.part_index) fail(KK_EINVAL, "bad peer rank %d", rank);
-  if (kind == kPeerPool && m->plan.mode != KK_MODE_BROADCAST && !(m->plan.mode == KK_MODE_SCATTER && (m->plan.flags & KK_LOAD_SCATTER_EXCHANGE)))
+  const LoadShape& S = m->shape;
+  if (kind == kPeerRaw && S.order != LoadOrder::kRaw) fail(KK_ESTATE, "raw peer attach needs a KK_FANOUT_RAW model");
+  if (kind == kPeerSlice && S.order != LoadOrder::kPull) fail(KK_ESTATE, "slice attach needs a KK_FANOUT_PULL model");
+  if (!S.multi_proc) fail(KK_ESTATE, "peer attach needs a multi-process (part_count > 1) model");
+  if (rank < 0 || rank >= S.n_parts || rank == S.rank) fail(KK_EINVAL, "bad peer rank %d", rank);
+  // a multi-process SCATTER model with KK_LOAD_SCATTER_EXCHANGE is the one that has an xdst table
+  if (kind == kPeerPool && m->plan.mode != KK_MODE_BROADCAST && !S.xdst)
     fail(KK_ESTATE, "peer attach only applies to BROADCAST models and to SCATTER models loaded with KK_LOAD_SCATTER_EXCHANGE");
   PeerBuf& b = m->peer[kind][rank];
   {
     std::lock_guard<std::mutex> g(m->peer_mu);
     if (b.ptr) fail(KK_ESTATE, "peer rank %d already attached", rank);
   }
-  KK_CUDA(cudaSetDevice(m->ctx->devs[(size_t)m->dev_idx[0]].ordinal));
+  KK_CUDA(cudaSetDevice(m->ctx->devs[0].ordinal));
   void* p = nullptr;
   if (is_ipc) {
     cudaIpcMemHandle_t h;
@@ -1038,8 +999,8 @@ void model_peer_detach_all(kk_model* m) {
 }
 
 int model_local_device(kk_model* m, int ordinal) {
-  for (size_t li = 0; li < m->dev_idx.size(); ++li)
-    if (m->ctx->devs[(size_t)m->dev_idx[li]].ordinal == ordinal) return (int)li;
+  for (size_t li = 0; li < m->pools.size(); ++li)
+    if (m->ctx->devs[li].ordinal == ordinal) return (int)li;
   fail(KK_EINVAL, "device %d holds no pool of this model", ordinal);
 }
 
@@ -1048,7 +1009,7 @@ void model_pool_ipc_handle(kk_model* m, int li, void* handle_out) {
   if (m->pool_handle_cache.size() < m->pools.size()) m->pool_handle_cache.resize(m->pools.size());
   auto& c = m->pool_handle_cache[(size_t)li];
   if (c.empty()) {
-    KK_CUDA(cudaSetDevice(m->ctx->devs[(size_t)m->dev_idx[(size_t)li]].ordinal));
+    KK_CUDA(cudaSetDevice(m->ctx->devs[(size_t)li].ordinal));
     cudaIpcMemHandle_t h;
     KK_CUDA(cudaIpcGetMemHandle(&h, m->pools[(size_t)li].ptr));
     static_assert(sizeof h == KK_IPC_HANDLE_BYTES, "ipc handle size");
@@ -1060,18 +1021,18 @@ void model_pool_ipc_handle(kk_model* m, int li, void* handle_out) {
 static std::string build_manifest(kk_model* m, int li);
 std::string model_manifest(kk_model* m, int li) {
   std::lock_guard<std::mutex> g(m->export_mu);
-  if (m->manifest_cache.size() < m->dev_idx.size()) m->manifest_cache.resize(m->dev_idx.size());
+  if (m->manifest_cache.size() < m->pools.size()) m->manifest_cache.resize(m->pools.size());
   auto& c = m->manifest_cache[(size_t)li];
   if (c.empty()) c = build_manifest(m, li);
   return c;
 }
 
 static std::string build_manifest(kk_model* m, int li) {
-  const auto& pl = m->plan.placement_of_part(m->local_parts[(size_t)li]);
+  const auto& pl = m->plan.placement_of_part(m->shape.local_parts[(size_t)li]);
   const auto& T = m->plan.index.tensors;
   std::ostringstream o;
   // "device" is the ordinal in THIS process (diagnostics only); a consumer in another process or container finds the GPU by its UUID / PCI bus id
-  const int ordinal = m->ctx->devs[(size_t)m->dev_idx[(size_t)li]].ordinal;
+  const int ordinal = m->ctx->devs[(size_t)li].ordinal;
   char bus[32] = "", uuid[48] = "";
   try {
     device_identity(ordinal, bus, sizeof bus, uuid, sizeof uuid);
@@ -1098,33 +1059,28 @@ static std::string build_manifest(kk_model* m, int li) {
 std::string model_stats(kk_model* m) {
   std::ostringstream o;
   o.precision(9);
+  const std::vector<int>& local_parts = m->shape.local_parts;
   uint64_t src = 0, out = 0;
-  for (size_t li = 0; li < m->local_parts.size(); ++li) {
-    const PartPlan& pp = m->plan.parts[(size_t)m->local_parts[li]];
+  for (size_t li = 0; li < local_parts.size(); ++li) {
+    const PartPlan& pp = m->plan.parts[(size_t)local_parts[li]];
     src += pp.src_bytes;
     out += pp.out_bytes;
   }
   o << "{\"n_tensors\":" << m->plan.index.tensors.size() << ",\"n_shards\":" << m->plan.index.shards.size()
-    << ",\"file_bytes\":" << m->plan.file_bytes << ",\"pool_bytes\":" << m->plan.pool_bytes_of_part(m->local_parts[0])
+    << ",\"file_bytes\":" << m->plan.file_bytes << ",\"pool_bytes\":" << m->plan.pool_bytes_of_part(local_parts[0])
     << ",\"n_parts\":" << m->plan.n_parts << ",\"local_src_bytes\":" << src << ",\"local_out_bytes\":" << out
     << ",\"index_s\":" << m->t_index << ",\"plan_s\":" << m->t_plan << ",\"alloc_s\":" << m->t_alloc << ",\"load_s\":" << m->t_load
     << ",\"n_loads\":" << m->n_loads << ",\"readers\":{\"threads\":" << m->rd_threads << ",\"slot_wait_s\":" << m->rd_wait_ns.load() / 1e9 << ",\"pread_s\":" << m->rd_pread_ns.load() / 1e9
     << ",\"issue_s\":" << m->rd_issue_ns.load() / 1e9 << ",\"drain_s\":" << m->rd_drain_ns.load() / 1e9 << ",\"files_open_s\":" << m->t_files_open << ",\"files_close_s\":" << m->t_files_close << "},\"load_gbps\":" << (m->t_load > 0 ? (double)src / m->t_load / 1e9 : 0.0) << ",\"parts\":[";
-  for (size_t li = 0; li < m->local_parts.size(); ++li) {
-    const int part = m->local_parts[li];
+  for (size_t li = 0; li < local_parts.size(); ++li) {
+    const int part = local_parts[li];
     const PartPlan& pp = m->plan.parts[(size_t)part];
-    // pool range this part produces (contiguous for SINGLE/BROADCAST because pool order == file order)
-    uint64_t lo = UINT64_MAX, hi = 0;
-    for (auto& s : pp.segs) {
-      if (s.op == KK_OP_ROWSPLIT) continue;  // lands in every pool; not part of this rank's contiguous range
-      lo = std::min(lo, s.dst_off);
-      hi = std::max(hi, s.dst_off + seg_out_extent(s));
-    }
-    if (lo == UINT64_MAX) lo = 0;
+    uint64_t lo, hi;
+    part_pool_range(m->plan, part, lo, hi);
     uint64_t tiles = 0;
     for (auto& ch : pp.chunks) tiles += ch.n_tiles;
     if (li) o << ",";
-    o << "{\"part\":" << part << ",\"device\":" << m->ctx->devs[(size_t)m->dev_idx[li]].ordinal << ",\"chunks\":" << pp.chunks.size()
+    o << "{\"part\":" << part << ",\"device\":" << m->ctx->devs[li].ordinal << ",\"chunks\":" << pp.chunks.size()
       << ",\"segs\":" << pp.segs.size() << ",\"tiles\":" << tiles << ",\"src_bytes\":" << pp.src_bytes << ",\"out_bytes\":" << pp.out_bytes
       << ",\"pool_lo\":" << lo << ",\"pool_hi\":" << hi << ",\"seconds\":" << (li < m->t_part.size() ? m->t_part[li] : 0.0) << "}";
   }
@@ -1137,21 +1093,23 @@ std::string model_stats(kk_model* m) {
 // ---------------------------------------------------------------------------------------------
 void model_stage_resident(kk_model* m) {
   std::lock_guard<std::mutex> op(m->op_mu);
-  if (!is_raw(m)) m->images.clear();
+  const bool raw = m->shape.order == LoadOrder::kRaw;
+  const std::vector<int>& local_parts = m->shape.local_parts;
+  if (!raw) m->images.clear();
   else if (m->images.empty()) fail(KK_ESTATE, "the raw image of this model has been released");
   FdSet fds(m->plan.index.shards, map_policy());
-  if (is_raw(m)) {  // RAW: the resident image IS the raw image; stage this process's own part(s), no fan-out
-    for (size_t li = 0; li < m->dev_idx.size(); ++li)
-      stage_image(m, (int)li, m->local_parts[li], fds, m->images[li].image.get(), m->img_off[(size_t)m->local_parts[li]]);
+  if (raw) {  // RAW: the resident image IS the raw image; stage this process's own part(s), no fan-out
+    for (size_t li = 0; li < local_parts.size(); ++li)
+      stage_image(m, (int)li, local_parts[li], fds, m->images[li].image.get(), m->img_off[(size_t)local_parts[li]]);
     return;
   }
-  std::vector<DeviceImage> images(m->dev_idx.size());
-  for (size_t li = 0; li < m->dev_idx.size(); ++li) {
-    const int ordinal = m->ctx->devs[(size_t)m->dev_idx[li]].ordinal;
-    const ImageLayout im = lay_out_image(m->plan, {m->local_parts[li]});
+  std::vector<DeviceImage> images(local_parts.size());
+  for (size_t li = 0; li < local_parts.size(); ++li) {
+    const int ordinal = m->ctx->devs[li].ordinal;
+    const ImageLayout im = lay_out_image(m->plan, {local_parts[li]});
     DeviceImage& R = images[li];
     R.image = DevBuf(ordinal, im.bytes ? im.bytes : 256, "the resident image");
-    stage_image(m, (int)li, m->local_parts[li], fds, R.image.get(), im.chunk_off[0]);
+    stage_image(m, (int)li, local_parts[li], fds, R.image.get(), im.chunk_off[0]);
     R.segs = upload_segs(ordinal, im.segs);
     R.launches = im.launches;
   }
@@ -1160,7 +1118,7 @@ void model_stage_resident(kk_model* m) {
 
 void model_unstage_resident(kk_model* m) {
   std::lock_guard<std::mutex> op(m->op_mu);
-  if (is_raw(m)) return;  // the raw image lives as long as a deferred RAW model does
+  if (m->shape.order == LoadOrder::kRaw) return;  // the raw image lives as long as a deferred RAW model does
   m->images.clear();
 }
 
@@ -1168,12 +1126,11 @@ void model_unstage_resident(kk_model* m) {
 // launches on every local device.
 void model_convert_resident(kk_model* m, float* ms_total, float* ms_per_launch, size_t cap, size_t* n_launches) {
   std::lock_guard<std::mutex> op(m->op_mu);
-  const size_t nl = m->dev_idx.size();
+  const size_t nl = m->pools.size();
   std::vector<std::vector<ConvertLaunch>> launches(nl);
-  std::vector<DevBuf> tables(nl);  // RAW: the fan-out launches' segment tables
-  if (is_raw(m)) {
+  if (m->shape.order == LoadOrder::kRaw) {
     if (m->images.empty()) fail(KK_ESTATE, "the raw image of this model has been released");
-    for (size_t li = 0; li < nl; ++li) raw_fanout_launch(m, (int)li, tables[li], launches[li]);
+    for (size_t li = 0; li < nl; ++li) raw_fanout_launch(m, (int)li, launches[li]);
   } else {
     if (m->images.size() != nl) fail(KK_ESTATE, "kk_stage_resident has not been called");
     for (size_t li = 0; li < nl; ++li) {

@@ -85,6 +85,8 @@ struct DeviceImage {
   DevBuf segs;      // every part's segments rebased onto the image
   std::vector<ImageLaunch> launches;
   DevBuf copy_segs;  // RAW: one COPY segment per chunk of every part, [kk_model::chunk_base[part] + ci]
+  DevBuf fanout_segs;  // RAW: the same for this device's own part, tile_begin running, as the one launch `fanout`
+  ImageLaunch fanout{};
 };
 
 // The pool of one local device: cudaMalloc memory in whole 2 MiB multiples, a VMM allocation, or an alias into kk_model::nvls.  Its plan
@@ -118,10 +120,7 @@ struct kk_model {
   kk_ctx* ctx = nullptr;
   std::string key;
   kk::Plan plan;
-  kk_load_opts opts{};
-  // local devices that hold a pool, as indices into ctx->devs; local_parts[i] is the plan part device i ingests
-  std::vector<int> dev_idx;
-  std::vector<int> local_parts;
+  kk::LoadShape shape;  // local device li (every per-device vector below) is ctx->devs[li]
   // KK_FANOUT_NVLS (one process, >= 2 devices): per-device VMM allocations bound to one multicast object; the pools alias them, and this is
   // declared before the pools so that it outlives them
   std::unique_ptr<kk::NvlsPools> nvls;
@@ -144,7 +143,6 @@ struct kk_model {
   kk::DevBuf slice_buf;
   uint64_t slice_base = 0;
   std::vector<std::pair<uint64_t, uint64_t>> part_range;  // [lo, hi) pool bytes every part produces
-  bool raw_staged = false;                      // stage 1 complete on this process since the last conversion
   // state
   std::mutex op_mu;  // serialises the data-moving calls on ONE model (kk_load_part, kk_convert_local, kk_*_resident) against each other
   std::mutex peer_mu;  // guards peer[]; slice attach takes only this lock: stage 1 of a PULL load never reads the slice table, so slice buffers may be attached WHILE kk_load_part runs
@@ -179,7 +177,7 @@ void model_export_slice(kk_model* m, void* handle_out, bool as_pointer);
 void model_convert_local(kk_model* m, float* ms_total);
 void model_probe_peer(kk_model* m, int rank, PeerKind kind, uint64_t& nbytes, float* ms);
 void model_peer_detach_all(kk_model* m);
-int model_local_device(kk_model* m, int ordinal);  // index into m->dev_idx or throws
+int model_local_device(kk_model* m, int ordinal);  // local device index (into ctx->devs) or throws
 std::string model_manifest(kk_model* m, int local);
 void model_pool_ipc_handle(kk_model* m, int local, void* handle_64B);  // cudaIpcGetMemHandle of the pool, once per model and device
 std::string model_stats(kk_model* m);

@@ -443,6 +443,48 @@ Plan build_plan(Index index, int mode, uint32_t flags, int n_parts, uint64_t chu
   return P;
 }
 
+LoadShape resolve_load_shape(const kk_load_opts& opts, int n_devices, bool peer_ok) {
+  LoadShape S;
+  S.multi_proc = opts.part_count > 1;
+  const int part_count = S.multi_proc ? opts.part_count : 1;
+  S.rank = S.multi_proc ? opts.part_index : 0;
+  if (S.rank < 0 || S.rank >= part_count || part_count > KK_MAX_DEVICES) fail(KK_EINVAL, "part %d of %d out of range", S.rank, part_count);
+  if (opts.mode < KK_MODE_SINGLE || opts.mode > KK_MODE_SCATTER) fail(KK_EINVAL, "unknown mode %d", opts.mode);
+  if (opts.fanout < KK_FANOUT_P2P || opts.fanout > KK_FANOUT_PULL) fail(KK_EINVAL, "unknown fanout %d", opts.fanout);
+  const bool bcast = opts.mode == KK_MODE_BROADCAST;
+  if (opts.fanout == KK_FANOUT_NVLS) {
+    // every "cannot do NVLS here" is KK_EUNSUPPORTED (the contract since the first ABI version), whatever the reason
+    if (!bcast) fail(KK_EUNSUPPORTED, "fan-out NVLS only applies to KK_MODE_BROADCAST");
+    if (S.multi_proc) fail(KK_EUNSUPPORTED, "fan-out NVLS needs one process owning all devices (sharing a multicast object across processes is not implemented)");
+    if (n_devices < 2) fail(KK_EUNSUPPORTED, "fan-out NVLS needs at least two devices in the context");
+  }
+  if (opts.fanout == KK_FANOUT_RAW && !bcast) fail(KK_EINVAL, "KK_FANOUT_RAW only applies to KK_MODE_BROADCAST");
+  if (opts.fanout == KK_FANOUT_PULL && !bcast) fail(KK_EINVAL, "KK_FANOUT_PULL only applies to KK_MODE_BROADCAST");
+  if (opts.fanout == KK_FANOUT_PULL && !S.multi_proc)
+    fail(KK_EINVAL, "KK_FANOUT_PULL is for one-process-per-GPU operation (part_count > 1); one process owning the GPUs fans out with P2P stores");
+  if (S.multi_proc && n_devices != 1) fail(KK_EINVAL, "multi-process parts need a one-device context (got %d devices)", n_devices);
+  if (S.multi_proc && opts.mode == KK_MODE_SINGLE) fail(KK_EINVAL, "KK_MODE_SINGLE cannot be split into parts");
+
+  S.n_parts = opts.mode == KK_MODE_SINGLE ? 1 : S.multi_proc ? part_count : n_devices;
+  if (S.multi_proc || opts.mode == KK_MODE_SINGLE) S.local_parts = {S.rank};
+  else
+    for (int i = 0; i < n_devices; ++i) S.local_parts.push_back(i);
+  S.xdst = opts.mode == KK_MODE_SCATTER && (opts.flags & KK_LOAD_SCATTER_EXCHANGE) && S.n_parts > 1;
+  S.peer_ok = peer_ok;
+  // one process, >= 2 devices and no stores between them: each device builds its whole pool itself
+  const bool replicas = bcast && !S.multi_proc && n_devices > 1 && (opts.fanout == KK_FANOUT_NONE || !peer_ok);
+  if (bcast) {
+    if (opts.fanout == KK_FANOUT_RAW) S.order = LoadOrder::kRaw;
+    else if (opts.fanout == KK_FANOUT_PULL) S.order = LoadOrder::kPull;
+    else if (opts.fanout == KK_FANOUT_NVLS) S.order = LoadOrder::kNvls;
+    else if (replicas) S.order = LoadOrder::kReplicas;
+    else if (opts.fanout == KK_FANOUT_P2P && (S.multi_proc || n_devices > 1)) S.order = LoadOrder::kPush;
+  }
+  S.every_part = replicas && S.order != LoadOrder::kRaw;  // RAW's stage 1 gathers the parts; its stage 2 converts all of them anyway
+  S.two_stage = S.multi_proc && (S.order == LoadOrder::kRaw || S.order == LoadOrder::kPull);
+  return S;
+}
+
 std::string plan_to_json(const Plan& P) {
   std::ostringstream o;
   o << "{\"mode\":" << P.mode << ",\"flags\":" << P.flags << ",\"n_parts\":" << P.n_parts << ",\"file_bytes\":" << P.file_bytes

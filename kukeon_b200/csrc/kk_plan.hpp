@@ -73,6 +73,34 @@ std::string plan_to_json(const Plan& P);
 // True when KK_LOAD_GPT2_CONV1D_T applies to this tensor.
 bool is_gpt2_conv1d(const TensorRec& t);
 
+// How a load moves its bytes between the devices.
+enum class LoadOrder {
+  kOwn,       // every local device converts its own plan part into its own pool, and nothing else (SINGLE, SCATTER, BROADCAST with no peer)
+  kReplicas,  // BROADCAST, one process, >= 2 devices that do not store into each other (KK_FANOUT_NONE, or no peer access): each converts every part
+  kPush,      // BROADCAST, KK_FANOUT_P2P: the convert kernel also stores into every other pool (the context's, or the attached ranks')
+  kNvls,      // BROADCAST, KK_FANOUT_NVLS: one multimem.st per vector through the multicast object the pools are bound to
+  kRaw,       // BROADCAST, KK_FANOUT_RAW: file bytes all-gathered into per-device raw images (stage 1), each converted locally (stage 2)
+  kPull,      // BROADCAST, KK_FANOUT_PULL: own part into the own pool and a slice buffer (stage 1), the peers' slices pulled in (stage 2)
+};
+
+// A load's options resolved against its context, once per model: every stage of the load switches on this.
+struct LoadShape {
+  LoadOrder order = LoadOrder::kOwn;
+  bool multi_proc = false;       // one rank of a one-process-per-GPU load (part_count > 1)
+  int rank = 0;                  // the plan part this process ingests when multi_proc, else 0
+  int n_parts = 1;               // plan parts: 1 for SINGLE, else the ranks or the context's devices
+  std::vector<int> local_parts;  // per local device li (context device li): the plan part it ingests
+  bool every_part = false;       // every local device converts every plan part: kReplicas, and kNvls without peer access
+  bool xdst = false;             // the scatter row exchange: every launch carries every rank's pool (ConvertLaunch::xdst)
+  bool peer_ok = false;          // the context's devices reach each other's memory
+  bool two_stage = false;        // loaded only once kk_convert_local has run (multi-process RAW and PULL)
+};
+
+// Validates opts against a context of n_devices devices (peer_ok: with peer access between all of them) and resolves the load's shape;
+// throws KK_EINVAL / KK_EUNSUPPORTED.  The checks that need the driver (NVLS support) or the plan (multimem, PULL's pool ranges) and
+// RAW's need for peer access (checked when stage 1 runs) stay with the load.
+LoadShape resolve_load_shape(const kk_load_opts& opts, int n_devices, bool peer_ok);
+
 // Pool bytes from s.dst_off on that segment s spans in each destination pool.  Copies, casts and block dequantisers fill that range; a
 // transpose spans its whole output tensor but stores only its own rows' columns of it, strided; KK_OP_ROWSPLIT spans nothing here (its
 // rows land in every rank's pool).
