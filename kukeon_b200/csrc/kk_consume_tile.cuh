@@ -1,10 +1,40 @@
-// Consumer dispatch of kk_convert_kernel: which per-lane body a tile runs and with which arguments, as ONE function the device and the host
-// both compile.  The kernel's consumer threads call it for every tile they do not bulk-store (t.bulk 1 and 3 stay in kk_kernels.cu), and
-// tests/emul plays all consumer threads of a tile through it, so the CPU tier checks this dispatch — the warp rotation, every op's template
-// arguments, the transposes' gather and the row-split byte fallback — and not a copy of it.  Primitives: those of kk_dequant.cuh.
+// The per-tile walk of a kk_convert_kernel launch, as functions the device and the host both compile: the copies the producer issues for
+// a tile (kk_load_tile), the bulk stores of the aligned copy and row-split tiles (kk_store_tile), and the consumer dispatch of every other
+// tile — which per-lane body it runs and with which arguments (kk_consume_tile).  tests/emul plays whole launches through them, so the
+// CPU tier checks this walk — the copies, the bulk-store pieces, the warp rotation, every op's template arguments, the transposes' gather
+// and the row-split byte fallback — and not a copy of it.  What only the hardware needs (mbarriers, proxy fences, bulk-group commits and
+// waits) stays in kk_kernels.cu.  Primitives: those of kk_dequant.cuh, and bulk_load / store_bulk / rowsplit_store_bulk below.
 #pragma once
 #include "kk_dequant.cuh"
 #include "kk_tile.h"
+
+// The producer's copies of tile load ld into stage S: one bulk copy (kind 1) or one per source row (kind 2), each through
+// bulk_load(S, stage offset, source offset from the launch's src base, bytes).  Arming the stage's mbarrier with ld.tx is the caller's.
+template <class Stage>
+KK_DQ_DEV void kk_load_tile(const KKTileLoad& ld, const Stage& S) {
+  if (ld.kind == 1) bulk_load(S, 0u, ld.g_off, ld.tx);
+  else if (ld.kind == 2)
+    for (uint32_t r = 0; r < ld.nrows; ++r) bulk_load(S, r * ld.spitch, ld.g_off + (uint64_t)r * ld.gpitch, ld.row_bytes);
+}
+
+// The bulk stores of a tile with t.bulk == 1 (aligned copy: the payload at pay to every destination pool, store_bulk(D, pool, offset,
+// stage address, bytes)) or t.bulk == 3 (aligned row-split exchange: one store per (row, rank) piece, rowsplit_store_bulk(L, rank, offset,
+// stage address, bytes)).  One lane issues them.  The destinations' type is a template parameter too, so that store_bulk and Dst::n are
+// looked up only where the function is used: an includer that plays consumer tiles alone need not bind them.
+template <class Dst, class Launch>
+KK_DQ_DEV void kk_store_tile(const Dst& D, const KKTileDesc& t, uint32_t pay, const Launch& L) {
+  if (t.bulk == 1) {
+#pragma unroll
+    for (int dd = 0; dd < KK_MAX_DST; ++dd)
+      if (dd < (int)D.n) store_bulk(D, dd, t.dst_off, pay, t.n_units);
+    return;
+  }
+  for (KKRowSplitWalk w = kk_rowsplit_walk(t); w.pos < w.end;) {
+    const KKRowSplitPiece p = kk_rowsplit_piece(t, w);
+    rowsplit_store_bulk(L, p.dst.j, p.dst.off, pay + p.src, p.len);
+    kk_rowsplit_advance(t, w, p.len);
+  }
+}
 
 // 2-D transpose tile (KK_OP_T_*): staged by the producer (t.bulk == 4) or, when a source row is not 16-byte aligned, gathered here.
 template <int ES, int CONV>

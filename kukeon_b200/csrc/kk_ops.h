@@ -68,7 +68,6 @@
 #define KK_T_ROW_BYTES 4096u     /* per staged row: 1024 32-bit or 2048 16-bit columns */
 #define KK_MAX_DST 8
 /* ConvertLaunch::flags */
-#define KK_LAUNCH_NO_BULK_STORE 0x1u  /* force the register path for aligned copies (A/B measurement) */
 #define KK_LAUNCH_MULTIMEM 0x2u       /* dst[0] is an NVLS multicast address: store with multimem.st */
 
 enum KKOp : uint32_t {

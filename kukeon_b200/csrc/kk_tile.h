@@ -24,10 +24,12 @@ static_assert(sizeof(KKTileDesc) == 64, "KKTileDesc");
 // What the producer issues for the tile.  kind 0: nothing (the consumers gather the tile themselves, or it is empty);
 // kind 1: one bulk copy of `tx` bytes from src + g_off (16-byte aligned) to the start of the stage;
 // kind 2: `nrows` bulk copies of `row_bytes` from src + g_off + r * gpitch to stage + r * spitch.  tx is always the total byte count.
+// pay: the payload bytes among them, from the descriptor's pay_off on; the rest of a kind-1 copy (tx - pay_off - pay, at most 15 bytes) is the
+// 16-byte rounding of the superset, which the consumers must not depend on.
 struct KKTileLoad {
   uint32_t kind, tx;
   uint64_t g_off;
-  uint32_t nrows, row_bytes, spitch, pad_;
+  uint32_t nrows, row_bytes, spitch, pay;
   uint64_t gpitch;
 };
 
@@ -35,7 +37,7 @@ struct KKTileLoad {
 // alignment matters); flags: ConvertLaunch::flags.
 static inline KK_HD void kk_make_tile(const KKSeg& seg, uint32_t t, uint64_t src_addr, uint32_t flags, KKTileDesc& d, KKTileLoad& ld) {
   d.op = seg.op; d.pay_off = 0; d.n_units = 0; d.bulk = 0; d.dst_off = 0; d.src_off = 0; d.C = 0; d.R = 0; d.col0 = 0; d.row0 = 0;
-  ld.kind = 0; ld.tx = 0; ld.g_off = 0; ld.nrows = 0; ld.row_bytes = 0; ld.spitch = 0; ld.pad_ = 0; ld.gpitch = 0;
+  ld.kind = 0; ld.tx = 0; ld.g_off = 0; ld.nrows = 0; ld.row_bytes = 0; ld.spitch = 0; ld.pay = 0; ld.gpitch = 0;
   uint32_t in_bytes = 0;  // source bytes of this tile (single-copy ops)
   uint64_t in_off = 0;    // their offset from the src base
   uint32_t t_es = 0;  // transposes: source element size
@@ -108,7 +110,7 @@ static inline KK_HD void kk_make_tile(const KKSeg& seg, uint32_t t, uint64_t src
     const uint32_t rb = nc * t_es;
     if (((src_addr + d.src_off) & 15u) == 0 && (row_pitch & 15u) == 0 && (rb & 15u) == 0) {
       d.bulk = 4;
-      ld.tx = nr * rb;
+      ld.tx = ld.pay = nr * rb;
       ld.g_off = d.src_off;
       if (nc == C) {  // the tile spans whole rows: they are contiguous in the source, one bulk copy brings all of them
         ld.kind = 1;
@@ -124,13 +126,19 @@ static inline KK_HD void kk_make_tile(const KKSeg& seg, uint32_t t, uint64_t src
     d.pay_off = mis;
     ld.kind = 1;
     ld.tx = (mis + in_bytes + 15u) & ~15u;
+    ld.pay = in_bytes;
     ld.g_off = in_off - mis;
-    if (seg.op == KK_OP_COPY && mis == 0 && (in_bytes & 15u) == 0 && !(flags & (KK_LAUNCH_NO_BULK_STORE | KK_LAUNCH_MULTIMEM))) d.bulk = 1;
+    if (seg.op == KK_OP_COPY && mis == 0 && (in_bytes & 15u) == 0 && !(flags & KK_LAUNCH_MULTIMEM)) d.bulk = 1;
     // row-split exchange: every (row, destination) piece must be a whole number of 16-byte units on both sides
-    if (seg.op == KK_OP_ROWSPLIT && mis == 0 && (seg.p0 & 15u) == 0 && (seg.p1 & 15u) == 0 && (in_bytes & 15u) == 0 && (seg.dst_off & 15u) == 0 &&
-        !(flags & KK_LAUNCH_NO_BULK_STORE))
+    if (seg.op == KK_OP_ROWSPLIT && mis == 0 && (seg.p0 & 15u) == 0 && (seg.p1 & 15u) == 0 && (in_bytes & 15u) == 0 && (seg.dst_off & 15u) == 0)
       d.bulk = 3;
   }
+}
+
+// The segment tile `tile` belongs to: the last one whose tile_begin is <= tile, searched forward from `cur` (a CTA's tiles only increase).
+static inline KK_HD uint32_t kk_tile_seg(const uint32_t* tile_begin, uint32_t n_segs, uint32_t cur, uint32_t tile) {
+  while (cur + 1 < n_segs && tile_begin[cur + 1] <= tile) ++cur;
+  return cur;
 }
 
 // Row-split exchange (KK_OP_ROWSPLIT) addressing, shared by the kernel's two consumers and tests/emul.  A tile holds n_units bytes of this

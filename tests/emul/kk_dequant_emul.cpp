@@ -1,14 +1,15 @@
-// Host emulation of kk_convert_kernel's consumer side.  TEST INFRASTRUCTURE ONLY.
+// Host replay of kk_convert_kernel launches.  TEST INFRASTRUCTURE ONLY.
 //
-// Compiles kukeon_b200/csrc/kk_consume_tile.cuh — the kernel's per-tile dispatch and the consumer bodies it calls, the exact
-// device source — with g++ by binding the handful of primitives they use (shared-memory loads, single-rounding fp32
-// arithmetic, bf16 packing, the stores) to plain C++, then plays all 16 consumer warps x 32 lanes of a tile through
-// kk_consume_tile (play_tile).  What this checks, on the CPU test tier, is the part of a consumer that is easy to get wrong
-// and cannot be seen by reading a formula: which op runs which body with which arguments, which lane reads which bytes of
-// which block and where its output bytes land.  The bindings are stricter than the hardware: a misaligned 16/32-bit shared
-// load, a read outside the staged tile, a store outside the tile's output window or two stores to the same 16 bytes all fail
-// the run.  It does not check PTX spelling or memory ordering; the -m gpu parity tests do.  The product never links this file
-// and has no CPU path.
+// Compiles kukeon_b200/csrc/kk_consume_tile.cuh — the kernel's per-tile walk (the producer's copies, the bulk stores, the consumer
+// dispatch) and the consumer bodies it calls, the exact device source — with g++ by binding the handful of primitives they use
+// (bulk copies, shared-memory loads, single-rounding fp32 arithmetic, bf16 packing, the stores) to plain C++, then plays whole
+// launches through it (kk_emul_launch), all 16 consumer warps x 32 lanes of every tile (play_tile).  What this checks, on the CPU
+// test tier, is the part of the kernel that is easy to get wrong and cannot be seen by reading a formula: which tile the producer
+// builds and which bytes it stages, which op runs which body with which arguments, which lane reads which bytes of which block
+// and where its output bytes land.  The bindings are stricter than the hardware: a misaligned copy, 16/32-bit shared load or
+// bulk store, a read outside the tile's staged payload, a store outside the pool or two stores to the same bytes all fail the
+// run.  It does not check PTX spelling or memory ordering; the -m gpu parity tests do.  The product never links this file and
+// has no CPU path.
 #include <cmath>
 #include <cstdint>
 #include <algorithm>
@@ -165,7 +166,7 @@ inline uint32_t bf16_rne(float f) {
 }
 inline uint32_t pack_bf16x2(float a, float b) { return bf16_rne(a) | (bf16_rne(b) << 16); }
 
-struct Dsts { int unused; };
+struct Dsts { uint32_t n; };  // destination pools: g.out, then g.more_out
 // hits[u] counts the BYTES stored into 16-byte unit u: 16 after exactly one vector store (or eight 2-byte tail stores)
 inline void store16_all(const Dsts&, uint64_t off, const uint4& v) {
   if (g.pass == 1) return;
@@ -214,6 +215,17 @@ inline void store4_all(const Dsts&, uint64_t off, uint32_t v) {  // one 32-bit e
   g.hits[off >> 4] += 4;
   memcpy(g.out + off, &v, 4);
   for (int i = 0; i < g.n_more; ++i) memcpy(g.more_out[i] + off, &v, 4);
+}
+// Bulk store of `bytes` from the stage to pool d (t.bulk == 1): 16-byte aligned at both ends and in size, inside the pool and the staged
+// payload (else 13).  Pool 0's hit counters count it like every other store.
+inline void store_bulk(const Dsts&, int d, uint64_t off, uint32_t src, uint32_t bytes) {
+  if ((off & 15u) || (src & 15u) || (bytes & 15u) || off + bytes > g.out_bytes || src + bytes > g.tile_bytes) { flag(13); return; }
+  if (d == 0)
+    for (uint32_t u = 0; u < bytes; u += 16) {
+      if (g.hits[(off + u) >> 4]) flag(4);
+      g.hits[(off + u) >> 4] += 16;
+    }
+  memcpy((d ? g.more_out[d - 1] : g.out) + off, g.tile + src, bytes);
 }
 inline uint4 lds128(uint32_t a) {
   uint4 v{0, 0, 0, 0};
@@ -265,8 +277,36 @@ inline void rowsplit_store1(const Launch& L, uint32_t j, uint64_t off, uint8_t v
   if (g.pass == 1) return;
   if (int rc = rowsplit_store(L, j, off, &v, 1)) flag(rc);
 }
+// Bulk store of one row-split piece (t.bulk == 3): 16-byte aligned at both ends and in size and not empty (else 14), inside the staged
+// payload (else 16), then rowsplit_store's checks.
+inline void rowsplit_store_bulk(const Launch& L, uint32_t j, uint64_t off, uint32_t src, uint32_t len) {
+  if ((off & 15u) || (src & 15u) || (len & 15u) || !len) { flag(14); return; }
+  if (src + len > g.tile_bytes) { flag(16); return; }
+  if (int rc = rowsplit_store(L, j, off, g.tile + src, len)) flag(rc);
+}
 // The consumer barrier: play_tile has every thread run its stage stores (pass 1) before any thread's consumer reads count (pass 2).
 inline void named_bar_consumers() {}
+
+constexpr uint64_t kSrcAddr = 0x100000;  // the launch's src base: only its alignment matters (256 bytes, like the staging buffers)
+constexpr uint32_t kStageBytes = KK_TILE_SRC_BYTES + KK_STAGE_PAD;
+// A stage as the producer's copies fill it from the staged chunk src[0, src_bytes).  slack: bytes at the end of the tile's copies that are
+// not payload (the 16-byte rounding of a kind-1 superset, tx - pay_off - pay; 0 for row copies).  issued: bytes copied so far.
+struct Stage {
+  uint8_t* buf;
+  const uint8_t* src;
+  uint64_t src_bytes;
+  uint32_t slack;
+  uint32_t* issued;
+};
+// One bulk copy: 16-byte aligned source, destination and size, inside the stage (else 10); it may read up to 15 bytes past the chunk, which
+// the planner leaves as slack (else 11), but only its rounding may lie there, never payload (else 19).  Bytes past the chunk stay poison.
+inline void bulk_load(const Stage& S, uint32_t so, uint64_t go, uint32_t bytes) {
+  if (((kSrcAddr + go) & 15u) || (so & 15u) || (bytes & 15u) || so + bytes > kStageBytes) { flag(10); return; }
+  if (go > S.src_bytes || go + bytes > S.src_bytes + 15) { flag(11); return; }
+  if (go + bytes > S.src_bytes + S.slack) { flag(19); return; }
+  memcpy(S.buf + so, S.src + go, (size_t)std::min<uint64_t>(bytes, S.src_bytes - go));
+  *S.issued += bytes;
+}
 
 #define KK_DQ_DEV static inline
 #define min(a, b) ((a) < (b) ? (a) : (b))
@@ -278,9 +318,8 @@ inline void named_bar_consumers() {}
 // complete before pass 2 reads it; it suppresses pool stores.  Pass 2 replays the shuffles and votes, rewrites the same stage bytes and
 // stores.  it: the tile counter the kernel's warp rotation reads.  traces / straces (when given) receive each thread's pass-2 16/32-bit
 // shared loads and 16-byte store offsets.
-void play_tile(const KKTileDesc& t, const Launch& L, uint32_t it, std::vector<std::vector<uint32_t>>* traces = nullptr,
-               std::vector<std::vector<uint64_t>>* straces = nullptr) {
-  const Dsts D{0};
+void play_tile(const Dsts& D, const KKTileDesc& t, const Launch& L, uint32_t it, std::vector<std::vector<uint32_t>>* traces,
+               std::vector<std::vector<uint64_t>>* straces) {
   for (g.pass = 1; g.pass <= 2; ++g.pass)
     for (int ctid = 0; ctid < kConsumerThreads; ++ctid) {
       g.warp = ctid >> 5;
@@ -323,203 +362,92 @@ void count_wavefronts(const std::vector<std::vector<uint32_t>>& traces, uint64_t
   }
 }
 
-// Run the consumer side of one tile of block or elementwise op `op` (KKOp): `nblk` units whose first byte sits at tile[pay_off], additionally
-// reporting (when stats is given) the shared-memory wavefronts of the 16/32-bit loads (stats[0]) against one per warp load instruction
-// (stats[1]).  The wavefronts are only meaningful when all lanes of a warp execute the same loads (full warps of a full tile); byte loads
-// (lds8) and vector loads (lds64 / lds128) are not traced.  out receives nblk * out_bytes_per_block bytes; hits (out_bytes/16 counters,
-// zeroed here) how often each 16-byte unit was stored.  Returns 0, a positive Emu::err code, or -1 for a transpose or row-split op.
-extern "C" int kk_emul_dequant_tile_stats(uint32_t op, const uint8_t* tile, uint32_t tile_bytes, uint32_t pay_off, uint32_t nblk, uint8_t* out,
-                                          uint64_t out_bytes, uint8_t* hits, uint64_t* stats) {
-  if (kk_is_transpose(op) || op == KK_OP_ROWSPLIT) return -1;
-  g = Emu{};
-  g.tile = tile; g.tile_bytes = tile_bytes; g.out = out; g.out_bytes = out_bytes; g.hits = hits;
-  memset(hits, 0, (out_bytes + 15) / 16);
-  std::vector<uint8_t> mask(out_bytes / 2 + 1, 0), bmask(out_bytes + 1, 0);
-  g.out_mask = mask.data();
-  g.byte_mask = bmask.data();
-  KKTileDesc t{};
-  t.op = op; t.pay_off = pay_off; t.n_units = nblk;
-  std::vector<std::vector<uint32_t>> traces((size_t)kConsumerThreads);
-  play_tile(t, Launch{}, 0, stats ? &traces : nullptr);
-  if (stats) {
-    stats[0] = stats[1] = 0;
-    count_wavefronts(traces, stats[0], stats[1]);
-  }
-  return g.err;
-}
-
-extern "C" int kk_emul_dequant_tile(uint32_t op, const uint8_t* tile, uint32_t tile_bytes, uint32_t pay_off, uint32_t nblk, uint8_t* out,
-                                    uint64_t out_bytes, uint8_t* hits) {
-  return kk_emul_dequant_tile_stats(op, tile, tile_bytes, pay_off, nblk, out, out_bytes, hits, nullptr);
-}
-
-// A whole segment the way the kernel walks it: the producer's per-tile arithmetic (kk_block_tile, the same function the
-// kernel calls), the 16-byte aligned superset its bulk copy brings into the stage (pay_off = source address & 15), then the
-// consumers.  `src` holds the segment's blocks; src_misalign (0..15) is the alignment class of its first byte in the staged
-// chunk.  out/hits cover units * out_bytes_per_block bytes.  Returns like kk_emul_dequant_tile.
-extern "C" int kk_emul_dequant_segment(uint32_t op, const uint8_t* src, uint64_t units, uint32_t src_misalign, uint8_t* out, uint64_t out_bytes,
-                                       uint8_t* hits) {
-  const KKBlockGeom gm = kk_block_geom(op);
-  if (!gm.block_bytes) return -1;
-  KKSeg seg{};
-  seg.op = op;
-  seg.units = units;
-  seg.src_off = src_misalign;  // pretend the launch's src base is 16-byte aligned and the segment starts here
-  memset(hits, 0, out_bytes / 16);
-  static thread_local uint8_t stage[KK_TILE_SRC_BYTES + KK_STAGE_PAD];
-  std::vector<uint8_t> mask(out_bytes / 2 + 1, 0), bmask(out_bytes + 1, 0);
-  const uint64_t n_tiles = kk_seg_tiles(op, units, 0);
-  for (uint64_t t = 0; t < n_tiles; ++t) {
-    const KKBlockTile bt = kk_block_tile(seg, (uint32_t)t);
-    const uint32_t mis = (uint32_t)(bt.in_off & 15u);
-    const uint32_t tx = (mis + bt.in_bytes + 15u) & ~15u;  // what the producer asks TMA for
-    if (tx > sizeof stage) return 5;
-    memset(stage, 0xEE, sizeof stage);
-    // bytes before the payload / after it come from the neighbouring source bytes on the GPU; the consumers must not depend on them
-    memcpy(stage + mis, src + (bt.in_off - src_misalign), bt.in_bytes);
-    g = Emu{};
-    g.tile = stage; g.tile_bytes = mis + bt.in_bytes; g.out = out; g.out_bytes = out_bytes; g.hits = hits;
-    g.out_mask = mask.data();
-    g.byte_mask = bmask.data();
-    KKTileDesc d{};
-    d.op = op; d.pay_off = mis; d.n_units = bt.n_blocks; d.dst_off = bt.dst_off;
-    play_tile(d, Launch{}, (uint32_t)t);
-    if (g.err) return g.err;
-  }
-  return 0;
-}
-
-// One transpose tile (KK_OP_T_*: 8 rows, compact rows) the way the
-// kernel runs it.  `src` points at source element (r0, c0) of a row-major [*, C] tensor of ES-byte elements; staged != 0 lays the tile out
-// as the producer's bulk copies do, staged == 0 runs the consumers' gather fallback first.  `dst` is the destination tensor's origin
-// ([C_total, R] row-major, 2-byte elements — 4-byte for KK_OP_T_B32), dst_bytes its size; hits as in kk_emul_dequant_tile over dst.
-// stats: [0] shared-memory wavefronts the consumers' loads need (one per distinct 4-byte word per bank per warp instruction), [1] the
-// ideal (one per warp load), [2] warp-level 16-byte store instructions, [3] distinct 128-byte lines and [4] distinct 32-byte sectors those
-// touch, summed over instructions (what the LSU / L2 see as transactions).
-extern "C" int kk_emul_t_tile(uint32_t op, const uint8_t* src, uint32_t C, uint32_t nr, uint32_t nc, uint32_t R, uint32_t col0, uint32_t row0,
-                              int staged, uint8_t* dst, uint64_t dst_bytes, uint8_t* hits, uint64_t* stats) {
-  if (!kk_is_transpose(op)) return -1;
-  const uint32_t es = kk_t_src_es(op);
-  if (nr > KK_T_ROWS || nc * es > KK_T_ROW_BYTES) return 5;
-  static thread_local uint8_t stage[KK_TILE_SRC_BYTES + KK_STAGE_PAD];
-  memset(stage, 0xEE, sizeof stage);
-  std::vector<uint8_t> mask(dst_bytes / 2 + 1, 0), bmask(dst_bytes + 1, 0);
-  memset(hits, 0, (dst_bytes + 15) / 16);
-  g = Emu{};
-  g.tile = stage; g.wtile = stage; g.tile_bytes = sizeof stage; g.out = dst; g.out_bytes = dst_bytes; g.hits = hits; g.out_mask = mask.data();
-  g.byte_mask = bmask.data();
-  KKTileDesc t{};
-  t.op = op; t.n_units = nr | (nc << 16); t.bulk = staged ? 4 : 0; t.C = C; t.R = R; t.col0 = col0; t.row0 = row0;
-  if (staged)
-    for (uint32_t r = 0; r < nr; ++r) memcpy(stage + r * nc * es, src + (uint64_t)r * C * es, (size_t)nc * es);
-  Launch L;
-  L.src = src;
-  std::vector<std::vector<uint32_t>> traces((size_t)kConsumerThreads);
-  std::vector<std::vector<uint64_t>> straces((size_t)kConsumerThreads);
-  play_tile(t, L, 0, &traces, &straces);
-  uint64_t wavefronts = 0, ideal = 0, st_instr = 0, st_lines = 0, st_sectors = 0;
-  count_wavefronts(traces, wavefronts, ideal);
-  for (int w = 0; w < kConsumerWarps; ++w) {
+// 16-byte store transactions of per-lane store traces: the k-th recorded store of every lane of a warp is one warp instruction; it touches
+// as many 128-byte lines and 32-byte sectors as its lanes' offsets span (what the LSU / L2 see as transactions).  Adds to instr / lines /
+// sectors.
+void count_stores(const std::vector<std::vector<uint64_t>>& traces, uint64_t& instr, uint64_t& lines, uint64_t& sectors) {
+  for (size_t w = 0; w + 31 < traces.size(); w += 32) {
     size_t longest = 0;
-    for (int l = 0; l < 32; ++l) longest = std::max(longest, straces[(size_t)(32 * w + l)].size());
-    for (size_t k = 0; k < longest; ++k) {  // likewise the k-th 16-byte store
-      std::vector<uint64_t> lines, sectors;
+    for (int l = 0; l < 32; ++l) longest = std::max(longest, traces[w + l].size());
+    for (size_t k = 0; k < longest; ++k) {
+      std::vector<uint64_t> ls, ss;
       for (int l = 0; l < 32; ++l) {
-        const auto& tr = straces[(size_t)(32 * w + l)];
+        const auto& tr = traces[w + l];
         if (k >= tr.size()) continue;
         const uint64_t ln = tr[k] >> 7, sc = tr[k] >> 5;
-        if (std::find(lines.begin(), lines.end(), ln) == lines.end()) lines.push_back(ln);
-        if (std::find(sectors.begin(), sectors.end(), sc) == sectors.end()) sectors.push_back(sc);
+        if (std::find(ls.begin(), ls.end(), ln) == ls.end()) ls.push_back(ln);
+        if (std::find(ss.begin(), ss.end(), sc) == ss.end()) ss.push_back(sc);
       }
-      if (lines.empty()) continue;
-      st_instr += 1;
-      st_lines += lines.size();
-      st_sectors += sectors.size();
+      if (ls.empty()) continue;
+      instr += 1;
+      lines += ls.size();
+      sectors += ss.size();
     }
   }
-  if (stats) { stats[0] = wavefronts; stats[1] = ideal; stats[2] = st_instr; stats[3] = st_lines; stats[4] = st_sectors; }
-  return g.err;
 }
 
-// A whole launch of kk_convert_kernel, tile by tile: resolve the tile's segment from tile_begin[] (as the producer does), kk_make_tile (the
-// function the kernel's producer calls), perform the bulk copies it asks for into a stage buffer with the hardware's constraints checked
-// (16-byte aligned source, destination and size; bytes issued == bytes announced), then the consumer side: the kernel's two bulk-store paths
-// (aligned copy, aligned row-split exchange), or every other tile through kk_consume_tile (play_tile) with the launch's tile counter.
-// src: the staged chunk (src base assumed 256-byte aligned like the staging buffers); dst[0..n_dst): destination pools of pool_bytes each;
-// hits / masks describe dst[0] and ACCUMULATE across calls (the caller zeroes them once per pool).
+// A whole launch of kk_convert_kernel, tile by tile, through the kernel's own functions: the segment lookup (kk_tile_seg), the tile
+// (kk_make_tile), its copies into a stage buffer (kk_load_tile, checked by bulk_load; the bytes issued must equal the bytes announced to the
+// mbarrier), then the consumer side — the bulk stores of aligned copy and row-split tiles (kk_store_tile), or every other tile through
+// kk_consume_tile (play_tile) with the launch's tile counter.  The consumers may read the payload only: the 16-byte rounding of a superset
+// behind it is out of range, or poison for lds32_slack.
+// src: the staged chunk of src_bytes (its base is taken as 256-byte aligned like the staging buffers); dst[0..n_dst): destination pools of
+// pool_bytes each; hits / masks describe dst[0] and ACCUMULATE across calls (the caller zeroes them once per pool).
 // xdst[0..n_xdst): the pool of every rank, for KK_OP_ROWSPLIT tiles (ConvertLaunch::xdst); xpool_bytes, xhits and xmask1 are each pool's
 // size, 16-byte hit counters and per-byte store mask, shared with the launches of the other ranks so that a byte stored twice across ranks
 // fails.  rs_tiles (may be null) accumulates the row-split tiles played: [0] by bulk stores (bulk == 3), [1] by the byte-granular consumer.
+// stats (may be null) receives, summed over the tiles played through play_tile: [0] the shared-memory wavefronts of the consumers' 16/32-bit
+// loads (count_wavefronts; meaningful when all lanes of a warp execute the same loads — byte and vector loads are not traced), [1] the ideal
+// (one per warp load), [2] warp-level 16-byte store instructions, [3] the 128-byte lines and [4] the 32-byte sectors they touch (count_stores).
+// Returns 0, a positive failure code, or -1 for a bad destination count.
 extern "C" int kk_emul_launch(const uint8_t* src, uint64_t src_bytes, const KKSeg* segs, uint32_t n_segs, uint32_t n_tiles, uint32_t flags,
                               uint8_t* const* dst, uint32_t n_dst, uint64_t pool_bytes, uint8_t* hits, uint8_t* mask2, uint8_t* mask1,
                               uint8_t* const* xdst, uint32_t n_xdst, const uint64_t* xpool_bytes, uint8_t* const* xhits, uint8_t* const* xmask1,
-                              uint64_t* rs_tiles) {
+                              uint64_t* rs_tiles, uint64_t* stats) {
   if (n_dst < 1 || n_dst > KK_MAX_DST) return -1;
   Launch L;
   L.src = src; L.xdst = xdst; L.n_xdst = n_xdst; L.xpool_bytes = xpool_bytes; L.xhits = xhits; L.xmask1 = xmask1;
-  static thread_local uint8_t stage[KK_TILE_SRC_BYTES + KK_STAGE_PAD];
-  const uint64_t src_addr = 0x100000;  // only the alignment of the src base matters
+  const Dsts D{n_dst};
+  static thread_local uint8_t stage[kStageBytes];
+  std::vector<uint32_t> tile_begin(n_segs);
+  for (uint32_t i = 0; i < n_segs; ++i) tile_begin[i] = segs[i].tile_begin;
+  std::vector<std::vector<uint32_t>> traces(stats ? kConsumerThreads : 0);
+  std::vector<std::vector<uint64_t>> straces(stats ? kConsumerThreads : 0);
+  if (stats) memset(stats, 0, 5 * sizeof *stats);
   uint32_t cur = 0;
   for (uint32_t tile = 0; tile < n_tiles; ++tile) {
-    while (cur + 1 < n_segs && segs[cur + 1].tile_begin <= tile) ++cur;
+    cur = kk_tile_seg(tile_begin.data(), n_segs, cur, tile);
     const KKSeg& seg = segs[cur];
     if (tile < seg.tile_begin) return 9;  // tile_begin[] not monotone from 0
     KKTileDesc d;
     KKTileLoad ld;
-    kk_make_tile(seg, tile - seg.tile_begin, src_addr, flags, d, ld);
+    kk_make_tile(seg, tile - seg.tile_begin, kSrcAddr, flags, d, ld);
     memset(stage, 0xEE, sizeof stage);
-    uint32_t staged = 0;
-    if (ld.kind == 1) {
-      if (((src_addr + ld.g_off) & 15u) || (ld.tx & 15u) || ld.tx > sizeof stage) return 10;
-      if (ld.g_off > src_bytes) return 11;
-      // the last tile of a chunk may over-read up to 15 bytes of slack behind the staged bytes (the planner leaves room for it)
-      const uint64_t avail = src_bytes - ld.g_off;
-      if (ld.tx > avail + 15) return 11;
-      memcpy(stage, src + ld.g_off, (size_t)std::min<uint64_t>(ld.tx, avail));
-      staged = ld.tx;
-    } else if (ld.kind == 2) {
-      uint32_t sum = 0;
-      for (uint32_t r = 0; r < ld.nrows; ++r) {
-        const uint64_t go = ld.g_off + (uint64_t)r * ld.gpitch;
-        const uint32_t so = r * ld.spitch;
-        if (((src_addr + go) & 15u) || (so & 15u) || (ld.row_bytes & 15u) || so + ld.row_bytes > sizeof stage) return 10;
-        if (go + ld.row_bytes > src_bytes) return 11;
-        memcpy(stage + so, src + go, ld.row_bytes);
-        sum += ld.row_bytes;
-        staged = std::max(staged, so + ld.row_bytes);
-      }
-      if (sum != ld.tx) return 12;  // the mbarrier would never complete (or complete early)
-    }
     g = Emu{};
-    g.tile = stage; g.wtile = stage; g.tile_bytes = ld.kind ? staged : (uint32_t)sizeof stage;
+    uint32_t issued = 0;
+    kk_load_tile(ld, Stage{stage, src, src_bytes, ld.tx - d.pay_off - ld.pay, &issued});
+    if (g.err) return g.err;
+    if (issued != ld.tx) return 12;  // the mbarrier would never complete (or complete early)
+    g.tile = stage; g.wtile = stage; g.tile_bytes = ld.kind ? d.pay_off + ld.pay : kStageBytes;
     g.out = dst[0]; g.out_bytes = pool_bytes; g.hits = hits; g.out_mask = mask2; g.byte_mask = mask1;
     g.n_more = (int)n_dst - 1;
     for (int i = 0; i < g.n_more; ++i) g.more_out[i] = dst[i + 1];
     g.src_end = src + src_bytes;
-    if (d.bulk == 1) {  // aligned verbatim copy: one bulk store from the stage to every pool
-      if ((d.dst_off & 15u) || (d.n_units & 15u) || (d.pay_off & 15u) || d.dst_off + d.n_units > pool_bytes) return 13;
-      for (uint32_t u = 0; u < d.n_units; u += 16) {
-        if (hits[(d.dst_off + u) >> 4]) return 4;
-        hits[(d.dst_off + u) >> 4] += 16;
-      }
-      for (uint32_t i = 0; i < n_dst; ++i) memcpy(dst[i] + d.dst_off, stage + d.pay_off, d.n_units);
-      continue;
-    }
     if (d.op == KK_OP_ROWSPLIT && (!d.C || !d.R)) return 18;  // the kernel would divide by zero
-    if (d.bulk == 3) {  // row-split exchange, aligned: one bulk store per (row, rank) piece, from warp 0 lane 0
-      for (KKRowSplitWalk w = kk_rowsplit_walk(d); w.pos < w.end;) {
-        const KKRowSplitPiece p = kk_rowsplit_piece(d, w);
-        const uint32_t s0 = d.pay_off + p.src;
-        if ((p.dst.off & 15u) || (s0 & 15u) || (p.len & 15u) || !p.len) return 14;
-        if (s0 + p.len > staged) return 16;
-        if (int rc = rowsplit_store(L, p.dst.j, p.dst.off, stage + s0, p.len)) return rc;
-        kk_rowsplit_advance(d, w, p.len);
-      }
-      if (rs_tiles) ++rs_tiles[0];
+    if (d.bulk == 1 || d.bulk == 3) {  // one lane bulk-stores the stage
+      kk_store_tile(D, d, d.pay_off, L);
+      if (g.err) return g.err;
+      if (d.bulk == 3 && rs_tiles) ++rs_tiles[0];
       continue;
     }
-    play_tile(d, L, tile);
+    play_tile(D, d, L, tile, stats ? &traces : nullptr, stats ? &straces : nullptr);
     if (g.err) return g.err;
+    if (stats) {
+      count_wavefronts(traces, stats[0], stats[1]);
+      count_stores(straces, stats[2], stats[3], stats[4]);
+      for (auto& v : traces) v.clear();
+      for (auto& v : straces) v.clear();
+    }
     if (d.op == KK_OP_ROWSPLIT && rs_tiles) ++rs_tiles[1];
   }
   return 0;

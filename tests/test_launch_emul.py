@@ -11,51 +11,24 @@ all launches, and nothing else may have been touched.
 Not covered here (GPU tests only): the mbarrier / proxy-fence protocol and anything about timing."""
 import ctypes as C
 import os
-import subprocess
 
 import numpy as np
 import pytest
 
 from kukeon_b200 import gpupool
 from oracle import oracle
-from tests import helpers
+from tests import helpers, kk_emul
+from tests.kk_emul import ERR, NO_EXCHANGE, KKSeg, Pools
 from tools import synth
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 G = os.path.join(_HERE, "golden")
 MB = 1 << 20
-ERR = {1: "shared load outside the staged bytes", 2: "misaligned shared load", 3: "store outside the pool / misaligned", 4: "pool bytes stored twice",
-       8: "codebook index out of range", 9: "tile_begin[] not monotone", 10: "bulk copy violates 16-byte alignment / size / stage capacity",
-       11: "bulk copy reads outside the staged chunk", 12: "bytes issued != bytes announced to the mbarrier", 13: "bulk store misaligned or outside the pool",
-       14: "row-split bulk piece: destination, stage offset or length not 16-byte aligned", 15: "row-split store outside the destination pool",
-       16: "row-split store reads outside the staged bytes", 17: "row-split store to a rank without a pool", 18: "row-split tile with zero row or slice bytes",
-       -1: "op not covered by the emulator"}
-
-
-class KKSeg(C.Structure):
-    _fields_ = [("src_off", C.c_uint64), ("dst_off", C.c_uint64), ("units", C.c_uint64), ("op", C.c_uint32), ("tile_begin", C.c_uint32),
-                ("p0", C.c_uint32), ("p1", C.c_uint32), ("p2", C.c_uint32), ("p3", C.c_uint32)]
 
 
 @pytest.fixture(scope="module")
 def emul():
-    subprocess.run(["make", "-C", os.path.join(_HERE, "emul"), "-s"], check=True)
-    L = C.CDLL(os.environ.get("KK_EMUL_LIB") or os.path.join(_HERE, "emul", "_build", "libkk_dequant_emul.so"))  # override: A/B variants below
-    L.kk_emul_launch.argtypes = [C.c_void_p, C.c_uint64, C.POINTER(KKSeg), C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(C.c_void_p), C.c_uint32, C.c_uint64,
-                                 C.c_void_p, C.c_void_p, C.c_void_p,
-                                 C.POINTER(C.c_void_p), C.c_uint32, C.POINTER(C.c_uint64), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_uint64)]
-    L.kk_emul_launch.restype = C.c_int
-    assert C.sizeof(KKSeg) == 48
-    return L
-
-
-class Pools:
-    def __init__(self, n, nbytes):
-        self.bufs = [np.full(nbytes, 0xCD, np.uint8) for _ in range(n)]
-        self.hits = np.zeros((nbytes + 15) // 16, np.uint8)
-        self.m2 = np.zeros(nbytes // 2 + 1, np.uint8)
-        self.m1 = np.zeros(nbytes + 1, np.uint8)
-        self.ptrs = (C.c_void_p * n)(*[b.ctypes.data for b in self.bufs])
+    return kk_emul.load()
 
 
 class Exchange:
@@ -66,9 +39,6 @@ class Exchange:
         self.args = ((C.c_void_p * n)(*[r.bufs[0].ctypes.data for r in ranks]), n, (C.c_uint64 * n)(*[r.bufs[0].size for r in ranks]),
                      (C.c_void_p * n)(*[r.hits.ctypes.data for r in ranks]), (C.c_void_p * n)(*[r.m1.ctypes.data for r in ranks]))
         self.tiles = (C.c_uint64 * 2)()
-
-
-NO_EXCHANGE = (None, 0, None, None, None)
 
 
 def play_part(L, plan, part, pools, flags=0, x=None):
@@ -82,7 +52,7 @@ def play_part(L, plan, part, pools, flags=0, x=None):
             segs = (KKSeg * len(ch["segs"]))(*[KKSeg(s["src_off"], s["dst_off"], s["units"], s["op"], s["tile_begin"], s["p0"], s["p1"], s["p2"], s["p3"])
                                               for s in ch["segs"]])
             rc = L.kk_emul_launch(buf.ctypes.data, buf.size, segs, len(ch["segs"]), ch["n_tiles"], flags, pools.ptrs, len(pools.bufs), pools.bufs[0].size,
-                                  pools.hits.ctypes.data, pools.m2.ctypes.data, pools.m1.ctypes.data, *(x.args if x else NO_EXCHANGE), x.tiles if x else None)
+                                  pools.hits.ctypes.data, pools.m2.ctypes.data, pools.m1.ctypes.data, *(x.args if x else NO_EXCHANGE), x.tiles if x else None, None)
             assert rc == 0, f"part {part}: {ERR.get(rc, rc)}"
     finally:
         for fh in fhs:
@@ -235,10 +205,10 @@ def test_the_replay_notices_a_wrong_plan(emul, tmp_path):
     s = ch["segs"][0]
     seg = (KKSeg * 1)(KKSeg(s["src_off"], s["dst_off"], s["units"], s["op"], 1, 0, 0, 0, 0))  # first tile has no segment
     pools = Pools(1, len(exp))
-    assert emul.kk_emul_launch(buf.ctypes.data, buf.size, seg, 1, ch["n_tiles"], 0, pools.ptrs, 1, len(exp), pools.hits.ctypes.data, pools.m2.ctypes.data, pools.m1.ctypes.data, *NO_EXCHANGE, None) == 9
+    assert emul.kk_emul_launch(buf.ctypes.data, buf.size, seg, 1, ch["n_tiles"], 0, pools.ptrs, 1, len(exp), pools.hits.ctypes.data, pools.m2.ctypes.data, pools.m1.ctypes.data, *NO_EXCHANGE, None, None) == 9
     seg = (KKSeg * 1)(KKSeg(s["src_off"], s["dst_off"], s["units"], s["op"], 0, 0, 0, 0, 0))
     pools = Pools(1, len(exp))
-    assert emul.kk_emul_launch(buf.ctypes.data, buf.size // 2, seg, 1, ch["n_tiles"], 0, pools.ptrs, 1, len(exp), pools.hits.ctypes.data, pools.m2.ctypes.data, pools.m1.ctypes.data, *NO_EXCHANGE, None) == 11
+    assert emul.kk_emul_launch(buf.ctypes.data, buf.size // 2, seg, 1, ch["n_tiles"], 0, pools.ptrs, 1, len(exp), pools.hits.ctypes.data, pools.m2.ctypes.data, pools.m1.ctypes.data, *NO_EXCHANGE, None, None) == 11
 
 
 # ---- property tests: random inventories through whole launches of the device code ---------------------------------------------------------
