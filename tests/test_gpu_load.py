@@ -244,6 +244,48 @@ def test_special_values_nan_inf_subnormal(pool, tmp_path):
         assert np.array_equal(g("bf16"), bf)
     finally:
         m.release()
+    # The same patterns off 16-byte alignment (the 8-wide cast paths that assemble their loads, F32 also off 4 bytes), and as GPT-2 Conv1D
+    # weights through the transposes (F32 / F16 -> bf16, and F32 kept as it is): a staged geometry (rows of whole 16-byte units, padded
+    # header) and a gathered one (odd columns, rows off 16 bytes).  Every file through a plain load, a poisoned streaming load and three
+    # poisoned resident conversions, the whole pool against the oracle.
+    def fill(n, pat):
+        return np.resize(pat, n)
+
+    def write(path, tensors, pad):
+        hdr, data = {}, b""
+        for name, dt, shape, arr in tensors:
+            raw = arr.tobytes()
+            hdr[name] = {"dtype": dt, "shape": shape, "data_offsets": [len(data), len(data) + len(raw)]}
+            data += raw
+        raw = json.dumps(hdr, separators=(",", ":")).encode()
+        helpers.write_raw_safetensors(path, raw + b" " * ((-(8 + len(raw))) % 16 if pad else 0), data)
+
+    for shift in (1, 4, 6):
+        p = str(tmp_path / f"special_off{shift}.safetensors")
+        write(p, [("pad", "U8", [shift], np.zeros(shift, np.uint8)), ("f32", "F32", [len(f32)], f32), ("f16", "F16", [len(f16) + 3], fill(len(f16) + 3, f16))], True)
+        assert [r["file_offset"] % 16 for r in oracle.index_path(p)[1]][1] == shift
+        load_and_check(pool, p)
+    T, K = gpupool.LOAD_GPT2_CONV1D_T, gpupool.LOAD_KEEP_F32
+    for (r, c), lead, pad in (((64, 1024), 16, True), ((63, 1041), 3, False)):  # staged: rows of 4096 / 2048 B at 16-byte boundaries
+        p = str(tmp_path / f"special_t{c}.safetensors")
+        write(p, [("x", "U8", [lead], np.zeros(lead, np.uint8)), ("h.0.attn.c_attn.weight", "F32", [r, c], fill(r * c, f32)),
+                  ("h.0.mlp.c_proj.weight", "F16", [r, c], fill(r * c, f16))], pad)
+        load_and_check(pool, p, flags=T)
+        load_and_check(pool, p, flags=T | K)
+    # FP8 widened to bf16: a tensor of 16k + r elements puts its last r elements on the single-element tail.  Three rounds of r = 1..15
+    # per format give 360 tail elements, which cycle through all 256 byte patterns; the 16-element groups before them are random.
+    tensors = []
+    for dt in ("F8_E4M3", "F8_E5M2"):
+        rs = list(range(1, 16)) * 3
+        tails = (np.arange(sum(rs)) % 256).astype(np.uint8)
+        at = 0
+        for k, r in enumerate(rs):
+            body = np.frombuffer(np.random.default_rng(k).bytes(16 * (1 + k % 5)), np.uint8)
+            tensors.append((f"{dt}.{k}", dt, [body.size + r], np.concatenate([body, tails[at:at + r]])))
+            at += r
+    p = str(tmp_path / "special_f8.safetensors")
+    write(p, tensors, True)
+    load_and_check(pool, p, flags=gpupool.LOAD_F8_TO_BF16)
     # Q4_K with non-finite / zero / subnormal super-block scales
     blocks = np.frombuffer(np.random.default_rng(1).bytes(144 * 64), np.uint8).reshape(64, 144).copy()
     specials = [0x7C00, 0xFC00, 0x7E00, 0x0000, 0x8000, 0x0001, 0x7BFF, 0x03FF]
