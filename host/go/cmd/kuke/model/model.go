@@ -19,14 +19,14 @@ type MockIndexerKey struct{}
 // Indexer is the narrow surface the subcommands use; satisfied by the cgo package and by per-test fakes.
 type Indexer interface {
 	Index(path string) ([]gpupool.TensorMeta, error)
-	Plan(path string, mode gpupool.Mode, flags uint32, gpus int) ([]byte, error)
+	Plan(path string, mode gpupool.Mode, flags uint32, gpus int, layers gpupool.Layers) ([]byte, error)
 }
 
 type cgoIndexer struct{}
 
 func (cgoIndexer) Index(path string) ([]gpupool.TensorMeta, error) { return gpupool.Index(path) }
-func (cgoIndexer) Plan(path string, mode gpupool.Mode, flags uint32, gpus int) ([]byte, error) {
-	return gpupool.Plan(path, mode, flags, gpus)
+func (cgoIndexer) Plan(path string, mode gpupool.Mode, flags uint32, gpus int, layers gpupool.Layers) ([]byte, error) {
+	return gpupool.Plan(path, mode, flags, gpus, layers)
 }
 
 func resolveIndexer(cmd *cobra.Command) Indexer {
@@ -57,11 +57,15 @@ type planSummary struct {
 	PoolBytesPerGPU   []uint64 `json:"poolBytesPerGpu"   yaml:"poolBytesPerGpu"`
 	IngestBytesPerGPU []uint64 `json:"ingestBytesPerGpu" yaml:"ingestBytesPerGpu"`
 	Tensors           int      `json:"tensors"           yaml:"tensors"`
+	Layers            []uint32 `json:"layers,omitempty"  yaml:"layers,omitempty"`
+	NLayers           uint64   `json:"nLayers,omitempty" yaml:"nLayers,omitempty"`
 }
 
 // planDoc mirrors the fields of kk_plan_describe's JSON the summary needs.
 type planDoc struct {
-	FileBytes uint64 `json:"file_bytes"`
+	FileBytes uint64   `json:"file_bytes"`
+	Layers    []uint32 `json:"layers"`
+	NLayers   uint64   `json:"n_layers"`
 	Layouts   []struct {
 		PoolBytes uint64            `json:"pool_bytes"`
 		Tensors   []json.RawMessage `json:"tensors"`

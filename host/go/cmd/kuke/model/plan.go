@@ -38,7 +38,17 @@ func NewPlanCmd() *cobra.Command {
 			if mode == gpupool.ModeSingle {
 				gpus = 1
 			}
-			raw, err := resolveIndexer(cmd).Plan(strings.TrimSpace(args[0]), mode, 0, gpus)
+			var layers gpupool.Layers
+			if s, _ := cmd.Flags().GetString("layers"); s != "" {
+				b, e, found := strings.Cut(s, ":")
+				lb, berr := strconv.ParseUint(b, 10, 32)
+				le, eerr := strconv.ParseUint(e, 10, 32)
+				if !found || berr != nil || eerr != nil || lb >= le {
+					return fmt.Errorf("invalid layer range: %s (expected B:E with integers 0 <= B < E)", s)
+				}
+				layers = gpupool.Layers{Begin: uint32(lb), End: uint32(le)}
+			}
+			raw, err := resolveIndexer(cmd).Plan(strings.TrimSpace(args[0]), mode, 0, gpus, layers)
 			if err != nil {
 				return err
 			}
@@ -56,7 +66,7 @@ func NewPlanCmd() *cobra.Command {
 			if uerr := json.Unmarshal(raw, &doc); uerr != nil {
 				return uerr
 			}
-			sum := planSummary{Path: args[0], Mode: strings.ToLower(modeName), GPUs: gpus, FileBytes: doc.FileBytes}
+			sum := planSummary{Path: args[0], Mode: strings.ToLower(modeName), GPUs: gpus, FileBytes: doc.FileBytes, Layers: doc.Layers, NLayers: doc.NLayers}
 			if len(doc.Layouts) > 0 {
 				sum.Tensors = len(doc.Layouts[0].Tensors)
 			}
@@ -79,13 +89,18 @@ func NewPlanCmd() *cobra.Command {
 					rows = append(rows, []string{strconv.Itoa(g), formatSize(int64(sum.IngestBytesPerGPU[g])), formatSize(int64(sum.PoolBytesPerGPU[g]))})
 				}
 				getshared.PrintTable(cmd, []string{"GPU", "INGESTS", "POOL"}, rows)
-				cmd.Printf("%d tensors, %s in the files, mode %s\n", sum.Tensors, formatSize(int64(sum.FileBytes)), sum.Mode)
+				stage := ""
+				if len(sum.Layers) == 2 {
+					stage = fmt.Sprintf(", layers %d-%d of %d", sum.Layers[0], sum.Layers[1]-1, sum.NLayers)
+				}
+				cmd.Printf("%d tensors, %s in the files, mode %s%s\n", sum.Tensors, formatSize(int64(sum.FileBytes)), sum.Mode, stage)
 				return nil
 			}
 		},
 	}
 	cmd.Flags().String("mode", "single", "Load mode: single, broadcast, scatter")
 	cmd.Flags().Int("gpus", 1, "Number of GPUs the load is planned for")
+	cmd.Flags().String("layers", "", "Pipeline stage B:E: plan only layers [B, E) of the checkpoint")
 	cmd.Flags().Bool("full", false, "yaml/json: print the whole plan (chunks, reads, segments) instead of the summary")
 	cmd.Flags().StringP("output", "o", "", "Output format (yaml, json, table). Default: table")
 	return cmd

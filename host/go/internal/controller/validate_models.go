@@ -10,6 +10,7 @@ package controller
 import (
 	"regexp"
 	"fmt"
+	"math"
 	"os"
 	"path/filepath"
 	"strings"
@@ -41,6 +42,7 @@ var modelOptionFlags = map[string]uint32{
 //   - target: absolute container path; empty means /run/kukeon/gpupool.
 //   - mode: "", single, broadcast, scatter (case-insensitive).
 //   - devices: distinct non-negative ordinals, at most 8; empty means every device of the daemon's pool.
+//   - layers: absent, or [begin, end) with 0 <= begin < end: the pipeline stage of the checkpoint this container mounts.
 //   - options: gpt2Conv1dTranspose, keepF32, f8ToBf16.
 var modelNameRE = regexp.MustCompile(`^[A-Za-z0-9][A-Za-z0-9._-]*$`)
 
@@ -106,15 +108,28 @@ func validateModels(in []intmodel.ModelMount) ([]intmodel.ModelMount, error) {
 			devSeen[d] = struct{}{}
 		}
 
+		if m.Layers != nil && (len(m.Layers) != 2 || m.Layers[0] < 0 || m.Layers[0] >= m.Layers[1] || int64(m.Layers[1]) > math.MaxUint32) {
+			return nil, fmt.Errorf("%w (model[%d] layers %v)", errdefs.ErrModelLayersInvalid, i, m.Layers)
+		}
+
 		for k := range m.Options {
 			if _, ok := modelOptionFlags[k]; !ok {
 				return nil, fmt.Errorf("%w (model[%d] option %q)", errdefs.ErrModelOptionUnknown, i, k)
 			}
 		}
 
-		out[i] = intmodel.ModelMount{Name: name, Source: src, Target: target, Mode: mode, Devices: append([]int(nil), m.Devices...), Options: m.Options}
+		out[i] = intmodel.ModelMount{Name: name, Source: src, Target: target, Mode: mode, Devices: append([]int(nil), m.Devices...), Options: m.Options,
+			Layers: append([]int(nil), m.Layers...)}
 	}
 	return out, nil
+}
+
+// modelLoadLayers turns the validated layers into the stage the load selects (the zero value: the whole checkpoint).
+func modelLoadLayers(m intmodel.ModelMount) gpupool.Layers {
+	if len(m.Layers) != 2 {
+		return gpupool.Layers{}
+	}
+	return gpupool.Layers{Begin: uint32(m.Layers[0]), End: uint32(m.Layers[1])}
 }
 
 // modelLoadFlags folds the validated options into kk_load_opts.flags.

@@ -27,6 +27,7 @@ var (
 	ErrModelTargetNotAbsolute    = errors.New("model target must be an absolute container path")
 	ErrModelModeUnknown          = errors.New("model mode is not recognized; expected \"\", \"single\", \"broadcast\", or \"scatter\"")
 	ErrModelDevicesInvalid       = errors.New("model devices must be distinct non-negative CUDA ordinals")
+	ErrModelLayersInvalid        = errors.New("model layers must be [begin, end): two non-negative integers with begin < end")
 	ErrModelOptionUnknown        = errors.New("model option is not recognized")
 	ErrModelRegistryNotSupported = errors.New("registry references are not supported; use an absolute host path as source")
 )

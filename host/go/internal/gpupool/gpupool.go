@@ -141,13 +141,21 @@ func Index(path string) ([]TensorMeta, error) {
 	return out, nil
 }
 
+// Layers selects a pipeline stage: layers [Begin, End) of the checkpoint (kk_load_opts.layer_begin / layer_end).  The zero value is
+// the whole checkpoint.  The library checks the range against the checkpoint and documents which outer tensors each stage keeps.
+type Layers struct {
+	Begin, End uint32
+}
+
 // Plan is the dry run behind `kuke model plan` (kk_plan_describe): JSON, CPU only.
-func Plan(path string, mode Mode, flags uint32, gpus int) ([]byte, error) {
+func Plan(path string, mode Mode, flags uint32, gpus int, layers Layers) ([]byte, error) {
 	cs := C.CString(path)
 	defer C.free(unsafe.Pointer(cs))
 	var o C.kk_load_opts
 	o.mode = C.int32_t(mode)
 	o.flags = C.uint32_t(flags)
+	o.layer_begin = C.uint32_t(layers.Begin)
+	o.layer_end = C.uint32_t(layers.End)
 	var need C.size_t
 	if err := call(func() C.int { return C.kk_plan_describe(nil, cs, &o, C.int(gpus), 0, nil, 0, &need) }); err != nil {
 		return nil, err
@@ -160,14 +168,16 @@ func Plan(path string, mode Mode, flags uint32, gpus int) ([]byte, error) {
 }
 
 // Load makes the checkpoint resident (or returns the already-resident copy with its refcount bumped): N concurrent StartCell
-// calls for the same model share one load.
-func (p *Pool) Load(path string, mode Mode, flags uint32) (*Model, error) {
+// calls for the same model share one load.  A pipeline stage (layers not zero) is a model of its own.
+func (p *Pool) Load(path string, mode Mode, flags uint32, layers Layers) (*Model, error) {
 	cs := C.CString(path)
 	defer C.free(unsafe.Pointer(cs))
 	var o C.kk_load_opts
 	o.mode = C.int32_t(mode)
 	o.fanout = C.KK_FANOUT_P2P
 	o.flags = C.uint32_t(flags)
+	o.layer_begin = C.uint32_t(layers.Begin)
+	o.layer_end = C.uint32_t(layers.End)
 	m := &Model{}
 	if err := call(func() C.int { return C.kk_load_ex(p.h, cs, &o, &m.h) }); err != nil {
 		return nil, err

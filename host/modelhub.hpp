@@ -127,6 +127,11 @@ class Model {
   kk_model* h_ = nullptr;
 };
 
+// Pipeline stage: layers [begin, end) of a checkpoint (kk_load_opts.layer_begin / layer_end); {0, 0} is the whole checkpoint.
+struct Layers {
+  uint32_t begin = 0, end = 0;
+};
+
 class Pool {
  public:
   explicit Pool(const Config& cfg) {
@@ -148,11 +153,14 @@ class Pool {
   void Close() {
     if (h_) { errdefs::check(kk_close(h_)); h_ = nullptr; }
   }
-  Model Load(const std::string& path, int mode = KK_MODE_SINGLE, int fanout = KK_FANOUT_P2P, uint32_t flags = 0) {
+  // layers: the pipeline stage [begin, end) to load; {0, 0} is the whole checkpoint.  A stage is a model of its own.
+  Model Load(const std::string& path, int mode = KK_MODE_SINGLE, int fanout = KK_FANOUT_P2P, uint32_t flags = 0, Layers layers = {}) {
     kk_load_opts o{};
     o.mode = mode;
     o.fanout = fanout;
     o.flags = flags;
+    o.layer_begin = layers.begin;
+    o.layer_end = layers.end;
     kk_model* m = nullptr;
     errdefs::check(kk_load_ex(h_, path.c_str(), &o, &m));
     return Model(m);
@@ -195,8 +203,9 @@ inline TensorIndex Pull(const std::string& path) {
   return ix;
 }
 
-inline gpupool::Model Load(gpupool::Pool& pool, const std::string& path, int mode = KK_MODE_SINGLE, uint32_t flags = 0) {
-  return pool.Load(path, mode, KK_FANOUT_P2P, flags);
+inline gpupool::Model Load(gpupool::Pool& pool, const std::string& path, int mode = KK_MODE_SINGLE, uint32_t flags = 0,
+                           gpupool::Layers layers = {}) {
+  return pool.Load(path, mode, KK_FANOUT_P2P, flags, layers);
 }
 
 struct OCIMount { std::string destination, type, source; std::vector<std::string> options; };

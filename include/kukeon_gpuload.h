@@ -123,7 +123,7 @@ typedef enum kk_fanout {
 /* 0x20 and 0x40 selected round 1's two candidate transpose geometries; the 8-row tiles won the A/B and are what KK_LOAD_GPT2_CONV1D_T uses now */
 
 typedef struct kk_ctx kk_ctx;     /* one per process (kukeond lifetime) */
-typedef struct kk_model kk_model; /* refcounted; one per (checkpoint identity, mode, flags) */
+typedef struct kk_model kk_model; /* refcounted; one per (checkpoint identity, mode, flags, layer range) */
 
 typedef struct kk_config {
   int32_t n_devices;                /* 1..KK_MAX_DEVICES */
@@ -167,7 +167,28 @@ typedef struct kk_load_opts {
    * devices need". In SCATTER mode part_index/part_count select which slice this rank keeps. */
   int32_t part_index;
   int32_t part_count;
-  uint32_t reserved[3];
+  /* Pipeline stage: load only layers [layer_begin, layer_end) of the checkpoint.  layer_end == 0 loads the whole checkpoint.
+   * A stage is a model of its own (a context may hold several stages of one file); kk_plan_describe takes the same range.
+   * The range is part of the model's identity as given: [0, n_layers) holds the same tensors as the whole checkpoint but is a
+   * separate model (its own pool, and a manifest with the stage keys), so a caller should use one form per checkpoint.
+   *   - The layer of a tensor is N in its first dotted component pair "<container>.<N>." with <container> one of layers / h / blk
+   *     and N all digits (model.layers.3.mlp.up_proj.weight, transformer.h.0.attn.c_attn.weight, blk.7.ffn_down_exps.weight).
+   *     The checkpoint has n_layers = 1 + the largest N.  Every layered tensor must belong to one stack (the same text up to and
+   *     including "<container>.") — two numbered stacks, e.g. model.layers. and vision_tower.encoder.layers., are KK_EUNSUPPORTED.
+   *   - A layered tensor is kept iff layer_begin <= N < layer_end.  Tensors without a layer go by name suffix:
+   *     embed_tokens.weight, token_embd.weight, wte.weight, wpe.weight to the first stage (layer_begin == 0);
+   *     lm_head.weight, lm_head.bias, the name output.weight, *norm.weight, *norm.bias, ln_f.weight, ln_f.bias to the last stage
+   *     (layer_end == n_layers); with no lm_head.weight and no output.weight (tied embeddings) the token embedding (not wpe)
+   *     goes to the last stage as well; every other tensor (e.g. rope_freqs.weight) to every stage.
+   *   - KK_EINVAL: layer_begin != 0 with layer_end == 0, layer_begin >= layer_end, layer_end > n_layers.  KK_EUNSUPPORTED: a range
+   *     on a checkpoint without layered tensors.  All are raised before any device is touched.
+   * The stage's tensors then load exactly as a checkpoint of only those tensors would, in every mode, fan-out and flag: shards and
+   * file offsets are unchanged, and no byte outside the stage is read.  Deployments: one process per GPU passes its stage plus its
+   * part_index / part_count within the stage's group and attaches that group's peers only; one process opens one kk_ctx per stage
+   * group, over disjoint devices. */
+  uint32_t layer_begin;
+  uint32_t layer_end;
+  uint32_t reserved;
 } kk_load_opts;
 
 typedef struct kk_model_info {

@@ -1,7 +1,9 @@
 """`kuke model …` — Python model of the CLI verbs row f3 of SURVEY.md §8(f) proposes, patterned on `kuke image` (cmd/kuke/image/*.go):
 
     python -m kukeon_b200.cli model pull <path> [-o table|yaml|json]          index a local checkpoint ("pull" is local-path only)
-    python -m kukeon_b200.cli model plan <path> [--mode M] [--gpus N] [-o …]  dry-run: pool layout and bytes per GPU, no device touched
+    python -m kukeon_b200.cli model plan <path> [--mode M] [--gpus N] [--layers B:E] [-o …]
+                                                                              dry-run: pool layout and bytes per GPU, no device touched;
+                                                                              --layers: only the pipeline stage of layers [B, E)
     python -m kukeon_b200.cli model validate <cell.yaml>                      check the `models:` entries of a Cell manifest
 
 Like `kuke image`, these verbs run in-process (pkg/api/kukeonv1/client.go:93-98): they need no daemon and no GPU — `pull` is
@@ -57,6 +59,14 @@ def parse_output(fmt: str) -> str:
     return f or "table"
 
 
+def parse_layers(s: str) -> List[int]:
+    """--layers B:E -> [B, E]; the library checks the range against the checkpoint."""
+    b, sep, e = s.partition(":")
+    if not (sep and b.isdigit() and e.isdigit() and int(b) < int(e)):
+        raise argparse.ArgumentTypeError(f"invalid layer range {s!r}: expected B:E with integers 0 <= B < E")
+    return [int(b), int(e)]
+
+
 def cmd_pull(args, out) -> int:
     recs = gpupool.index(args.path)
     shards = gpupool.index_shards(args.path)
@@ -76,18 +86,21 @@ def cmd_pull(args, out) -> int:
 def cmd_plan(args, out) -> int:
     flags = sum(schema.OPTION_FLAGS[o] for o in args.option or [])
     n = 1 if args.mode == "single" else args.gpus
-    plan = gpupool.plan_describe(args.path, mode=MODES[args.mode], flags=flags, n_parts=n)
+    plan = gpupool.plan_describe(args.path, mode=MODES[args.mode], flags=flags, n_parts=n, layers=args.layers)
     summary = {"path": args.path, "mode": args.mode, "gpus": n, "fileBytes": plan["file_bytes"],
                "poolBytesPerGpu": [lay["pool_bytes"] for lay in plan["layouts"]] if args.mode == "scatter" else [plan["layouts"][0]["pool_bytes"]] * n,
                "ingestBytesPerGpu": [p["src_bytes"] for p in plan["parts"]],
                "tensors": len(plan["layouts"][0]["tensors"])}
+    if args.layers:
+        summary["layers"], summary["nLayers"] = plan["layers"], plan["n_layers"]
     fmt = parse_output(args.output)
     if fmt != "table":
         emit(summary if not args.full else plan, fmt, out)
         return 0
     rows = [[str(g), format_size(summary["ingestBytesPerGpu"][g]), format_size(summary["poolBytesPerGpu"][g])] for g in range(n)]
     print_table(["GPU", "INGESTS", "POOL"], rows, out)
-    out.write(f"{summary['tensors']} tensors, {format_size(plan['file_bytes'])} in the files, mode {args.mode}\n")
+    stage = f", layers {plan['layers'][0]}-{plan['layers'][1] - 1} of {plan['n_layers']}" if args.layers else ""
+    out.write(f"{summary['tensors']} tensors, {format_size(plan['file_bytes'])} in the files, mode {args.mode}{stage}\n")
     return 0
 
 
@@ -128,6 +141,7 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--mode", choices=sorted(MODES), default="single")
     p.add_argument("--gpus", type=int, default=1)
     p.add_argument("--option", action="append", choices=sorted(schema.OPTION_FLAGS))
+    p.add_argument("--layers", type=parse_layers, metavar="B:E", help="pipeline stage: plan only layers [B, E) (half-open)")
     p.add_argument("--full", action="store_true", help="yaml/json: the whole plan (chunks, reads, segments) instead of the summary")
     p.add_argument("-o", "--output", default="")
     p.set_defaults(fn=cmd_plan)

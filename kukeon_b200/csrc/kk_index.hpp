@@ -29,6 +29,10 @@ struct Index {
   std::vector<std::string> shards;  // absolute paths
   std::vector<uint64_t> shard_bytes;
   std::vector<TensorRec> tensors;   // sorted by (shard, file_offset, name)
+  // select_layers (kk_plan.hpp): the tensors are the pipeline stage [layer_begin, layer_end) of a checkpoint of n_layers layers.
+  // layer_end == 0: the whole checkpoint.
+  uint32_t layer_begin = 0, layer_end = 0;
+  uint64_t n_layers = 0;
 };
 
 // Throws kk::Error.

@@ -757,7 +757,8 @@ kk_model* model_load(kk_ctx* c, const std::string& path, const kk_load_opts& opt
   }
 
   std::ostringstream ks;
-  ks << canon(path) << "|m" << opts.mode << "|f" << opts.fanout << "|x" << (opts.flags & ~KK_LOAD_DEFER) << "|p" << opts.part_index << "/" << opts.part_count;
+  ks << canon(path) << "|m" << opts.mode << "|f" << opts.fanout << "|x" << (opts.flags & ~KK_LOAD_DEFER) << "|p" << opts.part_index << "/" << opts.part_count
+     << "|l" << opts.layer_begin << ":" << opts.layer_end;
   const std::string key = ks.str();
 
   kk_model* m = nullptr;
@@ -781,7 +782,7 @@ kk_model* model_load(kk_ctx* c, const std::string& path, const kk_load_opts& opt
   const LoadShape& S = m->shape;
   try {
     double t0 = now_s();
-    Index ix = index_path(path);
+    Index ix = select_layers(index_path(path), opts.layer_begin, opts.layer_end);
     m->t_index = now_s() - t0;
     t0 = now_s();
     m->plan = build_plan(std::move(ix), opts.mode, opts.flags & ~KK_LOAD_DEFER, S.n_parts, c->slot_bytes);
@@ -1042,7 +1043,10 @@ static std::string build_manifest(kk_model* m, int li) {
   }
   o << "{\"apiVersion\":\"kukeon.gpupool/v1\",\"kind\":\"PoolManifest\",\"device\":" << ordinal << ",\"deviceUUID\":\"" << uuid << "\",\"pciBusId\":\"" << bus
     << "\",\"poolBytes\":" << m->pools[(size_t)li].bytes << ",\"mode\":" << m->plan.mode << ",\"format\":\"" << m->plan.index.format
-    << "\",\"align\":" << KK_POOL_ALIGN << ",\"tensors\":[";
+    << "\",\"align\":" << KK_POOL_ALIGN;
+  const Index& ix = m->plan.index;
+  if (ix.layer_end) o << ",\"layerBegin\":" << ix.layer_begin << ",\"layerEnd\":" << ix.layer_end << ",\"nLayers\":" << ix.n_layers;
+  o << ",\"tensors\":[";
   for (size_t i = 0; i < T.size(); ++i) {
     const DtypeInfo* di = dtype_info(pl[i].dtype);
     if (i) o << ",";

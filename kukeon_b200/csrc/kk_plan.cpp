@@ -285,6 +285,80 @@ uint32_t scatter_slice_dim(const TensorRec& t, int n_parts) {
   return dim;
 }
 
+namespace {
+
+// Layer of a tensor: the first dotted component pair "<container>.<N>." with <container> one of layers / h / blk and N all digits.
+// stack receives the name up to and including "<container>.", which names the numbered stack the layer belongs to.
+bool layer_of(const std::string& n, uint64_t& layer, std::string& stack) {
+  size_t c = 0;  // start of the current component
+  while (c < n.size()) {
+    const size_t dot = n.find('.', c);
+    if (dot == std::string::npos) return false;
+    const std::string comp = n.substr(c, dot - c);
+    if (comp == "layers" || comp == "h" || comp == "blk") {
+      const size_t d0 = dot + 1, d1 = n.find('.', d0);
+      if (d1 != std::string::npos && d1 > d0 &&
+          std::all_of(n.begin() + (long)d0, n.begin() + (long)d1, [](char ch) { return ch >= '0' && ch <= '9'; })) {
+        layer = 0;
+        for (size_t i = d0; i < d1; ++i) layer = std::min<uint64_t>(layer * 10 + (uint64_t)(n[i] - '0'), 0xFFFFFFFFull);  // beyond any layer_end
+        stack = n.substr(0, dot + 1);
+        return true;
+      }
+    }
+    c = dot + 1;
+  }
+  return false;
+}
+
+}  // namespace
+
+Index select_layers(Index ix, uint32_t begin, uint32_t end) {
+  if (end == 0 && begin == 0) return ix;
+  if (end == 0) fail(KK_EINVAL, "layer range [%u, 0): layer_end 0 selects the whole checkpoint and takes layer_begin 0", begin);
+  if (begin >= end) fail(KK_EINVAL, "layer range [%u, %u) is empty", begin, end);
+  std::string stack;
+  uint64_t n_layers = 0;
+  bool has_head = false;
+  std::vector<uint64_t> layer(ix.tensors.size(), UINT64_MAX);  // UINT64_MAX: outer tensor
+  for (size_t i = 0; i < ix.tensors.size(); ++i) {
+    const std::string& n = ix.tensors[i].name;
+    std::string s;
+    if (layer_of(n, layer[i], s)) {
+      if (stack.empty()) stack = s;
+      else if (s != stack)
+        fail(KK_EUNSUPPORTED, "the checkpoint has two numbered layer stacks, \"%s\" and \"%s\" (tensor %s): a layer range cannot tell which to cut",
+             stack.c_str(), s.c_str(), n.c_str());
+      n_layers = std::max(n_layers, layer[i] + 1);
+    }
+    has_head = has_head || ends_with(n, "lm_head.weight") || n == "output.weight";
+  }
+  if (stack.empty()) fail(KK_EUNSUPPORTED, "layer range [%u, %u): the checkpoint has no tensor with a layer index (layers.N. / h.N. / blk.N.)", begin, end);
+  if (end > n_layers) fail(KK_EINVAL, "layer range [%u, %u) exceeds the checkpoint's %llu layers", begin, end, (unsigned long long)n_layers);
+  const bool first = begin == 0, last = end == n_layers;
+  auto any_suffix = [](const std::string& n, std::initializer_list<const char*> sufs) {
+    for (auto s : sufs)
+      if (ends_with(n, s)) return true;
+    return false;
+  };
+  std::vector<TensorRec> kept;
+  for (size_t i = 0; i < ix.tensors.size(); ++i) {
+    const std::string& n = ix.tensors[i].name;
+    bool keep;
+    if (layer[i] != UINT64_MAX) keep = layer[i] >= begin && layer[i] < end;
+    else if (any_suffix(n, {"embed_tokens.weight", "token_embd.weight", "wte.weight"})) keep = first || (last && !has_head);  // tied head
+    else if (ends_with(n, "wpe.weight")) keep = first;
+    else if (n == "output.weight" || any_suffix(n, {"lm_head.weight", "lm_head.bias", "norm.weight", "norm.bias", "ln_f.weight", "ln_f.bias"}))
+      keep = last;
+    else keep = true;  // e.g. GGUF rope_freqs.weight: every stage
+    if (keep) kept.push_back(std::move(ix.tensors[i]));
+  }
+  ix.tensors = std::move(kept);
+  ix.layer_begin = begin;
+  ix.layer_end = end;
+  ix.n_layers = n_layers;
+  return ix;
+}
+
 Plan build_plan(Index index, int mode, uint32_t flags, int n_parts, uint64_t chunk_bytes) {
   if (n_parts < 1 || n_parts > KK_MAX_DEVICES) fail(KK_EINVAL, "n_parts %d out of range", n_parts);
   if (mode != KK_MODE_SINGLE && mode != KK_MODE_BROADCAST && mode != KK_MODE_SCATTER) fail(KK_EINVAL, "unknown mode %d", mode);
@@ -488,7 +562,9 @@ LoadShape resolve_load_shape(const kk_load_opts& opts, int n_devices, bool peer_
 std::string plan_to_json(const Plan& P) {
   std::ostringstream o;
   o << "{\"mode\":" << P.mode << ",\"flags\":" << P.flags << ",\"n_parts\":" << P.n_parts << ",\"file_bytes\":" << P.file_bytes
-    << ",\"format\":\"" << P.index.format << "\",\"shards\":[";
+    << ",\"format\":\"" << P.index.format << "\"";
+  if (P.index.layer_end) o << ",\"layers\":[" << P.index.layer_begin << "," << P.index.layer_end << "],\"n_layers\":" << P.index.n_layers;
+  o << ",\"shards\":[";
   for (size_t i = 0; i < P.index.shards.size(); ++i) o << (i ? "," : "") << "\"" << json_escape(P.index.shards[i]) << "\"";
   o << "],\"layouts\":[";
   for (size_t L = 0; L < P.placements.size(); ++L) {

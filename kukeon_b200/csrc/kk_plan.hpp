@@ -67,6 +67,11 @@ Plan build_plan(Index index, int mode, uint32_t flags, int n_parts, uint64_t chu
 // SURVEY.md §8(a3.S5): column-parallel weights along dim 0, row-parallel weights along dim 1.
 uint32_t scatter_slice_dim(const TensorRec& t, int n_parts);
 
+// Pipeline stage [layer_begin, layer_end) of a checkpoint (the rule is documented next to kk_load_opts in kukeon_gpuload.h).  Keeps the
+// shard list, every kept record's shard index and the index order; layer_end == 0 with layer_begin == 0 returns the index unchanged.
+// Throws KK_EINVAL (empty or out-of-range range) and KK_EUNSUPPORTED (no layered tensors, or two numbered stacks).
+Index select_layers(Index index, uint32_t layer_begin, uint32_t layer_end);
+
 // JSON description of a plan (kk_plan_describe).
 std::string plan_to_json(const Plan& P);
 

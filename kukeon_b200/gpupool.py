@@ -85,7 +85,7 @@ class KKPlacement(C.Structure):
 
 class KKLoadOpts(C.Structure):
     _fields_ = [("mode", C.c_int32), ("fanout", C.c_int32), ("flags", C.c_uint32), ("part_index", C.c_int32),
-                ("part_count", C.c_int32), ("reserved", C.c_uint32 * 3)]
+                ("part_count", C.c_int32), ("layer_begin", C.c_uint32), ("layer_end", C.c_uint32), ("reserved", C.c_uint32)]
 
 
 class KKModelInfo(C.Structure):
@@ -235,11 +235,24 @@ def index_shards(path: str) -> List[str]:
     return out
 
 
-def plan_describe(path: str, mode: int = MODE_SINGLE, flags: int = 0, n_parts: int = 1, chunk_bytes: int = 0) -> dict:
-    """kk_plan_describe: pool layout + per-part chunk/segment lists, computed on the CPU."""
+def _set_layers(o: KKLoadOpts, layers: Optional[Sequence[int]]) -> None:
+    """layers=(begin, end): the pipeline stage [begin, end) (see kk_load_opts in kukeon_gpuload.h, which also validates the range);
+    None: the whole checkpoint."""
+    if layers is not None:
+        b, e = (int(x) for x in layers)
+        if not (0 <= b < 2**32 and 0 <= e < 2**32):
+            raise ErrInvalid(-1, f"layer range [{b}, {e}) does not fit kk_load_opts' uint32 fields")
+        o.layer_begin, o.layer_end = b, e
+
+
+def plan_describe(path: str, mode: int = MODE_SINGLE, flags: int = 0, n_parts: int = 1, chunk_bytes: int = 0,
+                  layers: Optional[Sequence[int]] = None) -> dict:
+    """kk_plan_describe: pool layout + per-part chunk/segment lists, computed on the CPU.  layers=(begin, end) describes that
+    pipeline stage only."""
     L = lib()
     o = KKLoadOpts()
     o.mode, o.flags = mode, flags
+    _set_layers(o, layers)
     need = C.c_size_t()
     _check(L.kk_plan_describe(None, os.fsencode(path), C.byref(o), n_parts, chunk_bytes, None, 0, C.byref(need)))
     buf = C.create_string_buffer(need.value)
@@ -431,9 +444,11 @@ class Pool:
         self.devices = list(devices)
 
     def load(self, path: str, mode: int = MODE_SINGLE, fanout: int = FANOUT_P2P, flags: int = 0, part_index: int = 0,
-             part_count: int = 0) -> Model:
+             part_count: int = 0, layers: Optional[Sequence[int]] = None) -> Model:
+        """kk_load_ex.  layers=(begin, end) loads the pipeline stage [begin, end) only, as a model of its own."""
         o = KKLoadOpts()
         o.mode, o.fanout, o.flags, o.part_index, o.part_count = mode, fanout, flags, part_index, part_count
+        _set_layers(o, layers)
         h = C.c_void_p()
         _check(lib().kk_load_ex(self._h, os.fsencode(path), C.byref(o), C.byref(h)))
         return Model(self, h.value)

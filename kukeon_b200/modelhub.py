@@ -36,7 +36,7 @@ import struct
 import tempfile
 import threading
 from dataclasses import dataclass, field
-from typing import Dict, List, Optional
+from typing import Dict, List, Optional, Sequence
 
 from . import gpupool
 from .gpupool import FANOUT_NONE, FANOUT_P2P, MODE_BROADCAST, MODE_SCATTER, MODE_SINGLE  # noqa: F401
@@ -68,11 +68,12 @@ def Pull(path: str) -> ModelRef:
 
 
 def Load(pool: gpupool.Pool, ref: ModelRef | str, mode: int = MODE_SINGLE, fanout: int = FANOUT_P2P, flags: int = 0,
-         part_index: int = 0, part_count: int = 0) -> gpupool.Model:
+         part_index: int = 0, part_count: int = 0, layers: Optional[Sequence[int]] = None) -> gpupool.Model:
     """Make the checkpoint resident in the pool(s).  Returns a refcounted Model; a second Load of the same
-    checkpoint returns the same resident copy with its count bumped."""
+    checkpoint returns the same resident copy with its count bumped.  layers=(begin, end) loads only that pipeline
+    stage, as a model of its own."""
     path = ref.path if isinstance(ref, ModelRef) else ref
-    return pool.load(path, mode=mode, fanout=fanout, flags=flags, part_index=part_index, part_count=part_count)
+    return pool.load(path, mode=mode, fanout=fanout, flags=flags, part_index=part_index, part_count=part_count, layers=layers)
 
 
 @dataclass

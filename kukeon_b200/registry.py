@@ -20,7 +20,7 @@ import os
 import shutil
 import tempfile
 from dataclasses import dataclass, field
-from typing import Dict, List, Optional
+from typing import Dict, List, Optional, Sequence
 
 FILE_NAME = ".kukeon-gpupool.json"
 API_VERSION = "kukeon.gpupool/v1"
@@ -79,14 +79,22 @@ class Entry:
     devices: List[int]
     shards: List[dict]
     mounts: List[str] = field(default_factory=list)  # staged <container>/gpupool directories
+    # pipeline stage [begin, end) the pool holds; None: the whole checkpoint.  A restarted daemon reloads this stage, not the whole
+    # model (which need not fit the devices).
+    layers: Optional[List[int]] = None
 
     def to_json(self) -> dict:
-        return dict(key=self.key, path=self.path, mode=self.mode, fileBytes=self.file_bytes, poolBytes=self.pool_bytes,
-                    devices=self.devices, shards=self.shards, mounts=self.mounts)
+        d = dict(key=self.key, path=self.path, mode=self.mode, fileBytes=self.file_bytes, poolBytes=self.pool_bytes,
+                 devices=self.devices, shards=self.shards, mounts=self.mounts)
+        if self.layers is not None:
+            d["layers"] = self.layers
+        return d
 
     @staticmethod
     def from_json(d: dict) -> "Entry":
-        return Entry(d["key"], d["path"], d["mode"], d["fileBytes"], d["poolBytes"], list(d["devices"]), list(d["shards"]), list(d.get("mounts", [])))
+        layers = d.get("layers")
+        return Entry(d["key"], d["path"], d["mode"], d["fileBytes"], d["poolBytes"], list(d["devices"]), list(d["shards"]), list(d.get("mounts", [])),
+                     None if layers is None else list(layers))
 
 
 class RegistryError(RuntimeError):
@@ -153,10 +161,11 @@ class PoolRegistry:
 
     # -- steady state --------------------------------------------------------------------------
     def record(self, key: str, path: str, mode: int, file_bytes: int, pool_bytes: int, devices: List[int], shards: List[str],
-               mount_dir: Optional[str] = None) -> Entry:
+               mount_dir: Optional[str] = None, layers: Optional[Sequence[int]] = None) -> Entry:
         e = self.entries.get(key)
         if e is None:
-            e = Entry(key, path, mode, file_bytes, pool_bytes, sorted(devices), shard_fingerprints(shards))
+            e = Entry(key, path, mode, file_bytes, pool_bytes, sorted(devices), shard_fingerprints(shards),
+                      layers=None if layers is None else list(layers))
             self.entries[key] = e
         if mount_dir and mount_dir not in e.mounts:
             e.mounts.append(mount_dir)

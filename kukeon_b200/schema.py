@@ -10,6 +10,7 @@ Proposed schema — `models[]` on a v1beta1 ContainerSpec, next to `volumes[]` (
             source: /models/llama-3-8b        # absolute host path: directory (index.json / *.safetensors / *.gguf) or one file
             mode: broadcast        # single | broadcast | scatter      (kk_mode; default single)
             devices: [0, 1]        # CUDA ordinals the agent may attach to (default: every device of the daemon's pool)
+            layers: [0, 16]        # pipeline stage: only layers [begin, end) of the checkpoint (default: all of them)
             target: /run/kukeon/gpupool       # absolute container path of the read-only manifest mount (default shown)
             options: {gpt2Conv1dTranspose: false, keepF32: false, f8ToBf16: false}
 
@@ -22,7 +23,7 @@ from __future__ import annotations
 import os
 import re
 from dataclasses import dataclass, field
-from typing import Dict, List, Optional
+from typing import Dict, List, Optional, Tuple
 
 from . import gpupool
 
@@ -45,6 +46,7 @@ class Err:
     ModelTargetNotAbsolute = "model target must be an absolute container path"
     ModelModeUnknown = 'model mode is not recognized; expected "", "single", "broadcast", or "scatter"'
     ModelDevicesInvalid = "model devices must be distinct non-negative CUDA ordinals"
+    ModelLayersInvalid = "model layers must be [begin, end): two non-negative integers with begin < end"
     ModelOptionUnknown = "model option is not recognized"
     ModelRegistryNotSupported = "registry references are not supported; use an absolute host path as source"
 
@@ -65,6 +67,7 @@ class ModelSpec:
     devices: List[int] = field(default_factory=list)
     target: str = DEFAULT_TARGET
     flags: int = 0
+    layers: Optional[Tuple[int, int]] = None  # pipeline stage [begin, end); None: the whole checkpoint
 
 
 def _q(s: str) -> str:
@@ -109,13 +112,19 @@ def validate_models(models: Optional[List[dict]], stat=os.stat) -> List[ModelSpe
         if not isinstance(devs, list) or any(isinstance(d, bool) or not isinstance(d, int) or d < 0 for d in devs) or len(set(devs)) != len(devs) \
                 or len(devs) > gpupool.KK_MAX_DEVICES:
             raise SchemaError(Err.ModelDevicesInvalid, f"model[{i}] devices {devs!r}")
+        layers = m.get("layers")
+        if layers is not None:
+            if not isinstance(layers, list) or len(layers) != 2 or any(isinstance(v, bool) or not isinstance(v, int) or not 0 <= v < 2**32 for v in layers) \
+                    or layers[0] >= layers[1]:
+                raise SchemaError(Err.ModelLayersInvalid, f"model[{i}] layers {layers!r}")
+            layers = (layers[0], layers[1])
         flags = 0
         for k, v in (m.get("options") or {}).items():
             if k not in OPTION_FLAGS:
                 raise SchemaError(Err.ModelOptionUnknown, f"model[{i}] option {_q(str(k))}")
             if v:
                 flags |= OPTION_FLAGS[k]
-        out.append(ModelSpec(name=name, source=src, mode=MODES[mode], devices=list(devs), target=target, flags=flags))
+        out.append(ModelSpec(name=name, source=src, mode=MODES[mode], devices=list(devs), target=target, flags=flags, layers=layers))
     return out
 
 
