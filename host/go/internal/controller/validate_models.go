@@ -33,6 +33,7 @@ var modelOptionFlags = map[string]uint32{
 	"gpt2Conv1dTranspose": gpupool.FlagGPT2Conv1DTranspose,
 	"keepF32":             gpupool.FlagKeepF32,
 	"f8ToBf16":            gpupool.FlagF8ToBF16,
+	"f16":                 gpupool.FlagF16,
 }
 
 // validateModels normalises and checks the models[] of one container.
@@ -43,7 +44,8 @@ var modelOptionFlags = map[string]uint32{
 //   - mode: "", single, broadcast, scatter (case-insensitive).
 //   - devices: distinct non-negative ordinals, at most 8; empty means every device of the daemon's pool.
 //   - layers: absent, or [begin, end) with 0 <= begin < end: the pipeline stage of the checkpoint this container mounts.
-//   - options: gpt2Conv1dTranspose, keepF32, f8ToBf16.
+//   - options: gpt2Conv1dTranspose, keepF32, f8ToBf16, f16 (every float tensor as fp16 instead of bf16, for fp16 engines and fp16
+//     checkpoints; a model apart from the bf16 load of the same source).
 var modelNameRE = regexp.MustCompile(`^[A-Za-z0-9][A-Za-z0-9._-]*$`)
 
 func validateModels(in []intmodel.ModelMount) ([]intmodel.ModelMount, error) {

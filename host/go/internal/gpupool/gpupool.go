@@ -35,6 +35,9 @@ const (
 	FlagGPT2Conv1DTranspose uint32 = C.KK_LOAD_GPT2_CONV1D_T
 	FlagKeepF32             uint32 = C.KK_LOAD_KEEP_F32
 	FlagF8ToBF16            uint32 = C.KK_LOAD_F8_TO_BF16
+	// FlagF16 stores every float output as IEEE fp16 instead of bf16 (F16 tensors verbatim, BF16 / F32 / GGUF blocks rounded once);
+	// the pool layout is that of the same load without it.  An f16 and a bf16 load of one file are two models.
+	FlagF16 uint32 = C.KK_LOAD_F16
 )
 
 type Config struct {

@@ -51,6 +51,12 @@ inline void check(int rc) {
 
 namespace gpupool {
 
+// Load flags (kk_load_opts.flags), the names the Go package gives them; the models[].options of a manifest map onto these.
+constexpr uint32_t kFlagGPT2Conv1DTranspose = KK_LOAD_GPT2_CONV1D_T;
+constexpr uint32_t kFlagKeepF32 = KK_LOAD_KEEP_F32;
+constexpr uint32_t kFlagF8ToBF16 = KK_LOAD_F8_TO_BF16;
+constexpr uint32_t kFlagF16 = KK_LOAD_F16;  // every float output as IEEE fp16 instead of bf16, same pool layout
+
 struct Config {
   std::vector<int> devices{0};
   uint64_t pool_bytes_per_device = 0;

@@ -121,6 +121,20 @@ typedef enum kk_fanout {
                                       verbatim in the pool — FP8 engines want the bytes, and the per-block scale tensors that FP8
                                       checkpoints carry are model-specific and are not applied here */
 /* 0x20 and 0x40 selected round 1's two candidate transpose geometries; the 8-row tiles won the A/B and are what KK_LOAD_GPT2_CONV1D_T uses now */
+#define KK_LOAD_F16 0x80u           /* store every float output as IEEE binary16 (KK_F16) instead of bf16.  The pool's layout, sizes and
+                                      offsets are exactly those of the same load without the flag; only the dtype of the float tensors differs:
+                                        F16                 verbatim (a copy: NaN payloads kept byte for byte)
+                                        BF16                cast to f16: round to nearest even, overflow -> +-inf, f16 subnormals kept
+                                        F32                 cast to f16 likewise (still F32 under KK_LOAD_KEEP_F32)
+                                        GGUF block types    the same fp32 arithmetic as the bf16 load, then one RNE rounding to f16
+                                        F8_E4M3 / F8_E5M2   verbatim; f16 under KK_LOAD_F8_TO_BF16 (exact, the hardware's FP8 -> f16 pair conversion)
+                                        GPT-2 transposes    F32 / BF16 -> f16, F16 moved verbatim
+                                        integers, bool, F64, sub-byte: verbatim
+                                      Every NaN a conversion produces is 0x7FFF.  Composes with every mode, fan-out, KK_LOAD_DEFER, parts,
+                                      pipeline stages and VMM pools.  KK_LOAD_SCATTER_EXCHANGE keeps applying to the tensors the pool holds byte
+                                      for byte, so under this flag an F16 checkpoint's row-parallel tensors use the exchange and a BF16
+                                      checkpoint's are gathered (as F32 tensors are).  Flags are part of a model's identity: an f16 and a bf16
+                                      load of one file are two models. */
 
 typedef struct kk_ctx kk_ctx;     /* one per process (kukeond lifetime) */
 typedef struct kk_model kk_model; /* refcounted; one per (checkpoint identity, mode, flags, layer range) */
@@ -148,7 +162,7 @@ typedef struct kk_tensor_meta {
 
 typedef struct kk_placement {
   int32_t device;             /* CUDA ordinal */
-  uint32_t dtype;             /* dtype in the pool (KK_BF16 for every float tensor by default) */
+  uint32_t dtype;             /* dtype in the pool (KK_BF16 for every float tensor by default, KK_F16 under KK_LOAD_F16; KK_F32 under KK_LOAD_KEEP_F32) */
   uint64_t pool_offset;       /* byte offset inside that device's pool, multiple of KK_POOL_ALIGN */
   uint64_t nbytes;            /* bytes in the pool */
   uint32_t n_dims;

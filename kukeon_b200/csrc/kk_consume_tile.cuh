@@ -37,7 +37,7 @@ KK_DQ_DEV void kk_store_tile(const Dst& D, const KKTileDesc& t, uint32_t pay, co
 }
 
 // 2-D transpose tile (KK_OP_T_*): staged by the producer (t.bulk == 4) or, when a source row is not 16-byte aligned, gathered here.
-template <int ES, int CONV>
+template <bool F16, int ES, int CONV>
 KK_DQ_DEV void run_t(const Dsts& D, const uint8_t* src, const KKTileDesc& t, uint32_t sbase, int ctid) {
   const uint32_t nr = t.n_units & 0xFFFFu, nc = t.n_units >> 16;
   uint32_t pitch = nc * ES;
@@ -46,13 +46,14 @@ KK_DQ_DEV void run_t(const Dsts& D, const uint8_t* src, const KKTileDesc& t, uin
     t_gather<ES>(src + t.src_off, sbase, pitch, nr, nc, t.C, ctid);
     named_bar_consumers();
   }
-  consume_t<ES, CONV>(D, sbase, pitch, nr, nc, t.R, t.col0, t.row0, t.dst_off, ctid);
+  consume_t<F16, ES, CONV>(D, sbase, pitch, nr, nc, t.R, t.col0, t.row0, t.dst_off, ctid);
 }
 
 // One tile t, staged at sbase with its payload at pay, for consumer thread ctid = 32 * cwarp + lane.  L is the launch (the kernel's
 // ConvertLaunch): transposes gather from L.src, and row-split bytes go to rowsplit_store1(L, ...).  it counts the tiles this CTA's consumers
-// have taken, and selects the warp rotation.
-template <class Launch>
+// have taken, and selects the warp rotation.  F16: the launch's output format (KK_LAUNCH_F16), which every converting body is instantiated
+// for; the op codes name the default, bf16 output, which is also the default instantiation.
+template <bool F16 = false, class Launch>
 KK_DQ_DEV void kk_consume_tile(const Dsts& D, const KKTileDesc& t, uint32_t sbase, uint32_t pay, const Launch& L, int cwarp, int lane, int ctid,
                                uint32_t it) {
   // Block ops deal a tile's blocks (or groups of 4 / 8) to the 16 warps round-robin, and a full tile is rarely a multiple of 16 groups: a Q4_K tile
@@ -69,37 +70,37 @@ KK_DQ_DEV void kk_consume_tile(const Dsts& D, const KKTileDesc& t, uint32_t sbas
       break;
     }
     case KK_OP_COPY: consume_copy(D, pay, t.n_units, t.dst_off, ctid); break;
-    case KK_OP_F32_BF16: consume_f32(D, pay, t.n_units, t.dst_off, ctid); break;
-    case KK_OP_F16_BF16: consume_f16(D, pay, t.n_units, t.dst_off, ctid); break;
-    case KK_OP_Q4K_BF16: consume_q4k(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
-    case KK_OP_Q8_0_BF16: consume_q8_0(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
-    case KK_OP_Q6K_BF16: consume_q6k(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
-    case KK_OP_Q4_0_BF16: consume_legacy32<KK_Q4_0_BLOCK_BYTES, false, false>(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
-    case KK_OP_Q4_1_BF16: consume_legacy32<KK_Q4_1_BLOCK_BYTES, true, false>(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
-    case KK_OP_Q5_0_BF16: consume_legacy32<KK_Q5_0_BLOCK_BYTES, false, true>(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
-    case KK_OP_Q5_1_BF16: consume_legacy32<KK_Q5_1_BLOCK_BYTES, true, true>(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
-    case KK_OP_Q2K_BF16: consume_q2k(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
-    case KK_OP_Q3K_BF16: consume_q3k(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
-    case KK_OP_Q5K_BF16: consume_q5k(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
-    case KK_OP_IQ4NL_BF16: consume_codebook32<KK_IQ4NL_BLOCK_BYTES, 0>(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
-    case KK_OP_MXFP4_BF16: consume_codebook32<KK_MXFP4_BLOCK_BYTES, 1>(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
-    case KK_OP_IQ4XS_BF16: consume_iq4xs(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
-    case KK_OP_IQ2XXS_BF16: consume_iq2xxs(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
-    case KK_OP_IQ2XS_BF16: consume_iq2xs(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
-    case KK_OP_IQ2S_BF16: consume_iq2s(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
-    case KK_OP_IQ3XXS_BF16: consume_iq3xxs(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
-    case KK_OP_IQ3S_BF16: consume_iq3s(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
-    case KK_OP_IQ1S_BF16: consume_iq1s(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
-    case KK_OP_IQ1M_BF16: consume_iq1m(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
-    case KK_OP_TQ1_0_BF16: consume_tq1_0(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
-    case KK_OP_TQ2_0_BF16: consume_tq2_0(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
-    case KK_OP_NVFP4_BF16: consume_nvfp4(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
-    case KK_OP_F8E4M3_BF16: consume_f8<false>(D, pay, t.n_units, t.dst_off, ctid); break;
-    case KK_OP_F8E5M2_BF16: consume_f8<true>(D, pay, t.n_units, t.dst_off, ctid); break;
-    case KK_OP_T_F32_BF16: run_t<4, 1>(D, L.src, t, sbase, ctid); break;
-    case KK_OP_T_F16_BF16: run_t<2, 2>(D, L.src, t, sbase, ctid); break;
-    case KK_OP_T_B16: run_t<2, 0>(D, L.src, t, sbase, ctid); break;
-    case KK_OP_T_B32: run_t<4, 3>(D, L.src, t, sbase, ctid); break;
+    case KK_OP_F32_BF16: consume_f32<F16>(D, pay, t.n_units, t.dst_off, ctid); break;
+    case KK_OP_F16_BF16: consume_f16<F16>(D, pay, t.n_units, t.dst_off, ctid); break;
+    case KK_OP_Q4K_BF16: consume_q4k<F16>(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
+    case KK_OP_Q8_0_BF16: consume_q8_0<F16>(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
+    case KK_OP_Q6K_BF16: consume_q6k<F16>(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
+    case KK_OP_Q4_0_BF16: consume_legacy32<F16, KK_Q4_0_BLOCK_BYTES, false, false>(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
+    case KK_OP_Q4_1_BF16: consume_legacy32<F16, KK_Q4_1_BLOCK_BYTES, true, false>(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
+    case KK_OP_Q5_0_BF16: consume_legacy32<F16, KK_Q5_0_BLOCK_BYTES, false, true>(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
+    case KK_OP_Q5_1_BF16: consume_legacy32<F16, KK_Q5_1_BLOCK_BYTES, true, true>(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
+    case KK_OP_Q2K_BF16: consume_q2k<F16>(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
+    case KK_OP_Q3K_BF16: consume_q3k<F16>(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
+    case KK_OP_Q5K_BF16: consume_q5k<F16>(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
+    case KK_OP_IQ4NL_BF16: consume_codebook32<F16, KK_IQ4NL_BLOCK_BYTES, 0>(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
+    case KK_OP_MXFP4_BF16: consume_codebook32<F16, KK_MXFP4_BLOCK_BYTES, 1>(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
+    case KK_OP_IQ4XS_BF16: consume_iq4xs<F16>(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
+    case KK_OP_IQ2XXS_BF16: consume_iq2xxs<F16>(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
+    case KK_OP_IQ2XS_BF16: consume_iq2xs<F16>(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
+    case KK_OP_IQ2S_BF16: consume_iq2s<F16>(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
+    case KK_OP_IQ3XXS_BF16: consume_iq3xxs<F16>(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
+    case KK_OP_IQ3S_BF16: consume_iq3s<F16>(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
+    case KK_OP_IQ1S_BF16: consume_iq1s<F16>(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
+    case KK_OP_IQ1M_BF16: consume_iq1m<F16>(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
+    case KK_OP_TQ1_0_BF16: consume_tq1_0<F16>(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
+    case KK_OP_TQ2_0_BF16: consume_tq2_0<F16>(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
+    case KK_OP_NVFP4_BF16: consume_nvfp4<F16>(D, pay, t.n_units, t.dst_off, rwarp, lane); break;
+    case KK_OP_F8E4M3_BF16: consume_f8<F16, false>(D, pay, t.n_units, t.dst_off, ctid); break;
+    case KK_OP_F8E5M2_BF16: consume_f8<F16, true>(D, pay, t.n_units, t.dst_off, ctid); break;
+    case KK_OP_T_F32_BF16: run_t<F16, 4, 1>(D, L.src, t, sbase, ctid); break;
+    case KK_OP_T_F16_BF16: run_t<F16, 2, 2>(D, L.src, t, sbase, ctid); break;
+    case KK_OP_T_B16: run_t<F16, 2, 0>(D, L.src, t, sbase, ctid); break;
+    case KK_OP_T_B32: run_t<F16, 4, 3>(D, L.src, t, sbase, ctid); break;
     default: break;
   }
 }

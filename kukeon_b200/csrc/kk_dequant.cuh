@@ -11,8 +11,10 @@
 //     float    __fmul_rn / __fadd_rn / __fsub_rn one IEEE fp32 operation each — never contracted into an FMA, so results are
 //                                                bit-identical to gguf-py's numpy arithmetic (oracle/oracle.py)
 //     uint32_t pack_bf16x2(a, b)                 two floats -> bf16x2, RNE, NaN -> 0x7FFF
+//     uint32_t pack_f16x2(a, b)                  two floats -> f16x2, RNE, overflow -> +-inf, NaN -> 0x7FFF (the f16 instantiation:
+//                                                every body below is a template on the launch's output format, see pack2)
 //     void     store16_all(D, off, uint4)        16 output bytes to every destination pool
-//     void     store2_all(D, off, u16)           one bf16 (ragged tails); store4_all(D, off, u32): one 32-bit element (verbatim transposes)
+//     void     store2_all(D, off, u16)           one 16-bit output (ragged tails); store4_all(D, off, u32): one 32-bit element (verbatim transposes)
 //     uint4    lds128(a)                         16-byte aligned vector load
 //     uint32_t kk_f8x2_to_f16x2<E5M2>(u16)       two FP8 -> two fp16 (exact; cvt.rn.f16x2.e4m3x2 / .e5m2x2 on the device)
 //     float    kk_bits2f(u32)                    bit cast
@@ -30,10 +32,10 @@
 // index arithmetic of exactly this source is checked against the oracle on the CPU test tier.  That harness is test infrastructure:
 // the product has no CPU path.
 //
-// Lane mapping of the dequantisers, same for every type: a lane produces 8 consecutive weights = one 16-byte bf16 store; a warp
+// Lane mapping of the dequantisers, same for every type: a lane produces 8 consecutive weights = one 16-byte bf16 / fp16 store; a warp
 // iteration produces 512 contiguous output bytes (256-weight super-blocks: one block; 32-weight blocks: eight blocks).
 #pragma once
-#include "kk_consume_core.cuh"  // lds32_bytes, to_bf16
+#include "kk_consume_core.cuh"  // lds32_bytes, pack2, to16
 #include "kk_ops.h"
 
 // ---- loads of any alignment (blocks of 18..210 bytes are only 2-byte aligned inside a tile, or not at all) -----------
@@ -74,8 +76,9 @@ KK_DQ_DEV void lds64_funnel(uint32_t a, uint32_t& q0, uint32_t& q1) {
   q1 = kk_funnel_r(w1, w2, sh);
 }
 KK_DQ_DEV float lds_f16(uint32_t a) { return kk_h2f(lds16_any(a)); }
-KK_DQ_DEV void store_bf16x8(const Dsts& D, uint64_t off, const float (&y)[8]) {
-  store16_all(D, off, make_uint4(pack_bf16x2(y[0], y[1]), pack_bf16x2(y[2], y[3]), pack_bf16x2(y[4], y[5]), pack_bf16x2(y[6], y[7])));
+template <bool F16>
+KK_DQ_DEV void store_out8(const Dsts& D, uint64_t off, const float (&y)[8]) {  // eight outputs, one 16-byte store
+  store16_all(D, off, make_uint4(pack2<F16>(y[0], y[1]), pack2<F16>(y[2], y[3]), pack2<F16>(y[4], y[5]), pack2<F16>(y[6], y[7])));
 }
 
 // Byte k (0..3) of w minus BIAS as an exact float, without I2F: PRMT builds 0x4B0000bb = 2^23 + b, one FADD takes off 2^23 + BIAS.
@@ -92,6 +95,7 @@ KK_DQ_DEV uint32_t spread4(uint32_t x) { return ((x & 0xFu) * 0x00204081u) & 0x0
 
 // Q8_0 block (34 B): d f16 | qs[32] int8 -> 32 bf16, y = q * d in fp32 (gguf/quants.py Q8_0.dequantize_blocks).
 // Lane l of a warp handles elements 8*(l&3)..+8 of block (l>>2): 8 blocks and 512 contiguous output bytes per iteration.
+template <bool F16>
 KK_DQ_DEV void consume_q8_0(const Dsts& D, uint32_t pay, uint32_t nblk, uint64_t dst_off, int cwarp, int lane) {
 #pragma unroll 2
   for (uint32_t b0 = (uint32_t)cwarp * 8u; b0 < nblk; b0 += kConsumerWarps * 8u) {
@@ -109,7 +113,7 @@ KK_DQ_DEV void consume_q8_0(const Dsts& D, uint32_t pay, uint32_t nblk, uint64_t
       for (int e = 0; e < 8; ++e) y[e] = __fmul_rn(byte_to_float<128>(e < 4 ? q0 : q1, e & 3), d);
       if (b < nblk)
         store16_all(D, dst_off + (uint64_t)b * 64u + (uint32_t)(lane & 3) * 16u,
-                    make_uint4(pack_bf16x2(y[0], y[1]), pack_bf16x2(y[2], y[3]), pack_bf16x2(y[4], y[5]), pack_bf16x2(y[6], y[7])));
+                    make_uint4(pack2<F16>(y[0], y[1]), pack2<F16>(y[2], y[3]), pack2<F16>(y[4], y[5]), pack2<F16>(y[6], y[7])));
     }
   }
 }
@@ -118,6 +122,7 @@ KK_DQ_DEV void consume_q8_0(const Dsts& D, uint32_t pay, uint32_t nblk, uint64_t
 // element e = 32*g + i (g = 0..7): low nibble source ql[64*(g/4) + 32*(g%2) + i] >> 4*((g%4)/2), high 2 bits
 // qh[32*(g/4) + i] >> 2*(g%4); q = (lo | hi<<4) - 32; y = (d * scales[e/16]) * q, both products rounded to fp32.
 // Lane l handles the 8 elements e = 8l..8l+7 (g = l>>2, i = 8*(l&3)..+8): one block, 512 output bytes per warp iteration.
+template <bool F16>
 KK_DQ_DEV void consume_q6k(const Dsts& D, uint32_t pay, uint32_t nblk, uint64_t dst_off, int cwarp, int lane) {
   const int g = lane >> 2, i0 = 8 * (lane & 3);
   const uint32_t ql_off = 64u * (uint32_t)(g >> 2) + 32u * (uint32_t)(g & 1) + (uint32_t)i0;
@@ -139,7 +144,7 @@ KK_DQ_DEV void consume_q6k(const Dsts& D, uint32_t pay, uint32_t nblk, uint64_t 
 #pragma unroll
     for (int e = 0; e < 8; ++e) y[e] = __fmul_rn(dsc, byte_to_float<32>(e < 4 ? w0 : w1, e & 3));
     store16_all(D, dst_off + (uint64_t)b * 512u + (uint32_t)lane * 16u,
-                make_uint4(pack_bf16x2(y[0], y[1]), pack_bf16x2(y[2], y[3]), pack_bf16x2(y[4], y[5]), pack_bf16x2(y[6], y[7])));
+                make_uint4(pack2<F16>(y[0], y[1]), pack2<F16>(y[2], y[3]), pack2<F16>(y[4], y[5]), pack2<F16>(y[6], y[7])));
   }
 }
 
@@ -151,7 +156,7 @@ KK_DQ_DEV void consume_q6k(const Dsts& D, uint32_t pay, uint32_t nblk, uint64_t 
 // Element e < 16 is the LOW nibble of qs[e], element e >= 16 the HIGH nibble of qs[e-16]; bit 4 of element e is bit e of qh.
 // Lane l handles elements e0 = 8*(l&3) .. e0+7 of block (l>>2): they come from qs[e0 % 16 .. +8] (one nibble each) and
 // the byte (qh >> e0) & 0xFF.  Eight blocks and 512 contiguous output bytes per warp iteration.
-template <uint32_t BYTES, bool HAS_M, bool HAS_QH>
+template <bool F16, uint32_t BYTES, bool HAS_M, bool HAS_QH>
 KK_DQ_DEV void consume_legacy32(const Dsts& D, uint32_t pay, uint32_t nblk, uint64_t dst_off, int cwarp, int lane) {
   constexpr uint32_t kQhOff = HAS_M ? 4u : 2u;
   constexpr uint32_t kQsOff = kQhOff + (HAS_QH ? 4u : 0u);
@@ -181,7 +186,7 @@ KK_DQ_DEV void consume_legacy32(const Dsts& D, uint32_t pay, uint32_t nblk, uint
         if (HAS_M) y[e] = __fadd_rn(__fmul_rn(d, byte_to_float<0>(e < 4 ? q0 : q1, e & 3)), m);
         else y[e] = __fmul_rn(d, byte_to_float<(HAS_QH ? 16 : 8)>(e < 4 ? q0 : q1, e & 3));
       }
-      if (b < nblk) store_bf16x8(D, dst_off + (uint64_t)b * 64u + (uint32_t)(lane & 3) * 16u, y);
+      if (b < nblk) store_out8<F16>(D, dst_off + (uint64_t)b * 64u + (uint32_t)(lane & 3) * 16u, y);
     }
   }
 }
@@ -190,6 +195,7 @@ KK_DQ_DEV void consume_legacy32(const Dsts& D, uint32_t pay, uint32_t nblk, uint
 // Q2_K (84 B): scales[16] | qs[64] | d f16 | dmin f16  (gguf/quants.py:404-428).  Element e = 128h + 32s + i (h<2, s<4, i<32):
 // q = (qs[32h+i] >> 2s) & 3; 16-weight sub-block j = e/16: y = (d*(scales[j]&15))*q - dmin*(scales[j]>>4).
 // Lane l: h = l>>4, s = (l>>2)&3, i = 8*(l&3)..+8, j = l>>1.
+template <bool F16>
 KK_DQ_DEV void consume_q2k(const Dsts& D, uint32_t pay, uint32_t nblk, uint64_t dst_off, int cwarp, int lane) {
   const uint32_t q_off = 16u + 32u * (uint32_t)(lane >> 4) + 8u * (uint32_t)(lane & 3);
   const uint32_t sh = 2u * (uint32_t)((lane >> 2) & 3);
@@ -205,7 +211,7 @@ KK_DQ_DEV void consume_q2k(const Dsts& D, uint32_t pay, uint32_t nblk, uint64_t 
     float y[8];
 #pragma unroll
     for (int e = 0; e < 8; ++e) y[e] = __fsub_rn(__fmul_rn(dl, byte_to_float<0>(e < 4 ? q0 : q1, e & 3)), ml);
-    store_bf16x8(D, dst_off + (uint64_t)b * 512u + (uint32_t)lane * 16u, y);
+    store_out8<F16>(D, dst_off + (uint64_t)b * 512u + (uint32_t)lane * 16u, y);
   }
 }
 
@@ -213,6 +219,7 @@ KK_DQ_DEV void consume_q2k(const Dsts& D, uint32_t pay, uint32_t nblk, uint64_t 
 // low bits (qs[32*(g/4) + i] >> 2*(g%4)) & 3; q = low - 4 when bit g of hmask[i] is CLEAR, else low.  Scale k = e/16 is 6 bits:
 // low 4 = scales[k] & 15 (k<8) or scales[k-8] >> 4 (k>=8), high 2 = (scales[8 + k%4] >> 2*(k/4)) & 3, value - 32.
 // y = (d*scale_k)*q.  Lane l: g = l>>2, i = 8*(l&3)..+8, k = l>>1.
+template <bool F16>
 KK_DQ_DEV void consume_q3k(const Dsts& D, uint32_t pay, uint32_t nblk, uint64_t dst_off, int cwarp, int lane) {
   const uint32_t g = (uint32_t)(lane >> 2), i0 = 8u * (uint32_t)(lane & 3), k = (uint32_t)(lane >> 1);
   const uint32_t q_off = 32u + 32u * (g >> 2) + i0;
@@ -232,7 +239,7 @@ KK_DQ_DEV void consume_q3k(const Dsts& D, uint32_t pay, uint32_t nblk, uint64_t 
     float y[8];
 #pragma unroll
     for (int e = 0; e < 8; ++e) y[e] = __fmul_rn(dl, byte_to_float<4>(e < 4 ? w0 : w1, e & 3));
-    store_bf16x8(D, dst_off + (uint64_t)b * 512u + (uint32_t)lane * 16u, y);
+    store_out8<F16>(D, dst_off + (uint64_t)b * 512u + (uint32_t)lane * 16u, y);
   }
 }
 
@@ -240,16 +247,22 @@ KK_DQ_DEV void consume_q3k(const Dsts& D, uint32_t pay, uint32_t nblk, uint64_t 
 // q = ((qs[32*(j/2) + i] >> 4*(j%2)) & 15) | (((qh[i] >> j) & 1) << 4); (scale, min) of sub-block j packed as in Q4_K;
 // y = (d*sc_j)*q - dmin*m_j.  Implemented by consume_q5k in kk_consume_core.cuh: Q4_K's four-blocks-per-iteration quads with a fifth bit.
 
-// ---- §8(f4): FP8 (safetensors F8_E4M3 / F8_E5M2) widened to bf16, opt-in through KK_LOAD_F8_TO_BF16 -----------------------------
-// Elementwise and exact: FP8 -> fp16 with the hardware pair conversion, fp16 -> fp32 -> bf16 (RNE never rounds: every FP8 value
-// has at most 3 mantissa bits).  A thread turns 16 source bytes into two 16-byte stores; n = elements of the tile.
-template <bool E5M2>
-KK_DQ_DEV void f8x4_to_bf16x4(uint32_t w, uint32_t& o0, uint32_t& o1) {  // 4 FP8 in a word -> 2 + 2 bf16
+// ---- §8(f4): FP8 (safetensors F8_E4M3 / F8_E5M2) widened to bf16 or fp16, opt-in through KK_LOAD_F8_TO_BF16 -----------------------
+// Elementwise and exact: FP8 -> fp16 with the hardware pair conversion; for bf16 output then fp16 -> fp32 -> bf16 (RNE never rounds:
+// every FP8 value has at most 3 mantissa bits), for fp16 output the pair is stored as it is.  A thread turns 16 source bytes into two
+// 16-byte stores; n = elements of the tile.
+template <bool F16, bool E5M2>
+KK_DQ_DEV void f8x4_to_16x4(uint32_t w, uint32_t& o0, uint32_t& o1) {  // 4 FP8 in a word -> 2 + 2 outputs
   const uint32_t h0 = kk_f8x2_to_f16x2<E5M2>(w & 0xFFFFu), h1 = kk_f8x2_to_f16x2<E5M2>(w >> 16);
-  o0 = pack_bf16x2(kk_h2f(h0 & 0xFFFFu), kk_h2f(h0 >> 16));
-  o1 = pack_bf16x2(kk_h2f(h1 & 0xFFFFu), kk_h2f(h1 >> 16));
+  if (F16) {
+    o0 = h0;
+    o1 = h1;
+  } else {
+    o0 = pack_bf16x2(kk_h2f(h0 & 0xFFFFu), kk_h2f(h0 >> 16));
+    o1 = pack_bf16x2(kk_h2f(h1 & 0xFFFFu), kk_h2f(h1 >> 16));
+  }
 }
-template <bool E5M2>
+template <bool F16, bool E5M2>
 KK_DQ_DEV void consume_f8(const Dsts& D, uint32_t pay, uint32_t n, uint64_t dst_off, int ctid) {
   const uint32_t ngrp = n >> 4;  // 16 elements -> 32 B out
   const bool al = (pay & 15u) == 0;
@@ -264,14 +277,14 @@ KK_DQ_DEV void consume_f8(const Dsts& D, uint32_t pay, uint32_t n, uint64_t dst_
     }
     uint32_t o[8];
 #pragma unroll
-    for (int k = 0; k < 4; ++k) f8x4_to_bf16x4<E5M2>(w[k], o[2 * k], o[2 * k + 1]);
+    for (int k = 0; k < 4; ++k) f8x4_to_16x4<F16, E5M2>(w[k], o[2 * k], o[2 * k + 1]);
     store16_all(D, dst_off + ((uint64_t)g << 5), make_uint4(o[0], o[1], o[2], o[3]));
     store16_all(D, dst_off + ((uint64_t)g << 5) + 16u, make_uint4(o[4], o[5], o[6], o[7]));
   }
   const uint32_t tail = n & 15u, base = ngrp << 4;
   if ((uint32_t)ctid < tail) {
     const uint32_t h = kk_f8x2_to_f16x2<E5M2>(lds8(pay + base + (uint32_t)ctid));
-    store2_all(D, dst_off + 2ull * (base + (uint32_t)ctid), (uint16_t)(pack_bf16x2(kk_h2f(h & 0xFFFFu), 0.f) & 0xFFFFu));
+    store2_all(D, dst_off + 2ull * (base + (uint32_t)ctid), F16 ? (uint16_t)(h & 0xFFFFu) : (uint16_t)(pack_bf16x2(kk_h2f(h & 0xFFFFu), 0.f) & 0xFFFFu));
   }
 }
 
@@ -280,13 +293,13 @@ KK_DQ_DEV void consume_f8(const Dsts& D, uint32_t pay, uint32_t n, uint64_t dst_
 // by t_gather when the source rows are not 16-byte aligned).  Thread t takes columns t, t + 512, ...: its 8 loads walk DOWN one
 // column while the lanes of its warp sit side by side ALONG the row — consecutive shared-memory words, conflict-free whatever
 // the pitch — and the 8 converted values are the 8 * OES contiguous destination bytes dst[(col0 + c) * R + row0 .. + 8).
-template <int ES, int CONV>  // CONV: 0 verbatim 16-bit, 1 f32 -> bf16, 2 f16 -> bf16
+template <bool F16, int ES, int CONV>  // CONV: 0 verbatim 16-bit, 1 f32 -> output, 2 the other 16-bit float -> output (f16 -> bf16, bf16 -> f16)
 KK_DQ_DEV uint32_t t_pack2(uint32_t a, uint32_t b) {
-  if (CONV == 1) return pack_bf16x2(kk_bits2f(a), kk_bits2f(b));
-  if (CONV == 2) return pack_bf16x2(kk_h2f(a), kk_h2f(b));
+  if (CONV == 1) return pack2<F16>(kk_bits2f(a), kk_bits2f(b));
+  if (CONV == 2) return pack2<F16>(other16_to_f<F16>(a), other16_to_f<F16>(b));
   return (a & 0xFFFFu) | (b << 16);
 }
-template <int ES, int CONV>  // CONV 3: verbatim 32-bit (ES == 4, 4-byte outputs); otherwise 2-byte outputs
+template <bool F16, int ES, int CONV>  // CONV 3: verbatim 32-bit (ES == 4, 4-byte outputs); otherwise 2-byte outputs
 KK_DQ_DEV void consume_t(const Dsts& D, uint32_t sbase, uint32_t pitch, uint32_t nr, uint32_t nc, uint32_t R, uint32_t col0, uint32_t row0,
                          uint64_t dst_off, int ctid) {
   constexpr uint32_t OES = CONV == 3 ? 4u : 2u;
@@ -312,12 +325,12 @@ KK_DQ_DEV void consume_t(const Dsts& D, uint32_t sbase, uint32_t pitch, uint32_t
     } else if (vec) {
 #pragma unroll
       for (uint32_t g = 0; g < KK_T_ROWS / 8u; ++g)
-        store16_all(D, off + 16u * g, make_uint4(t_pack2<ES, CONV>(v[8 * g], v[8 * g + 1]), t_pack2<ES, CONV>(v[8 * g + 2], v[8 * g + 3]),
-                                                 t_pack2<ES, CONV>(v[8 * g + 4], v[8 * g + 5]), t_pack2<ES, CONV>(v[8 * g + 6], v[8 * g + 7])));
+        store16_all(D, off + 16u * g, make_uint4(t_pack2<F16, ES, CONV>(v[8 * g], v[8 * g + 1]), t_pack2<F16, ES, CONV>(v[8 * g + 2], v[8 * g + 3]),
+                                                 t_pack2<F16, ES, CONV>(v[8 * g + 4], v[8 * g + 5]), t_pack2<F16, ES, CONV>(v[8 * g + 6], v[8 * g + 7])));
     } else {
 #pragma unroll
       for (uint32_t k = 0; k < KK_T_ROWS; ++k)
-        if (k < nr) store2_all(D, off + 2u * k, (uint16_t)(t_pack2<ES, CONV>(v[k], 0u) & 0xFFFFu));
+        if (k < nr) store2_all(D, off + 2u * k, (uint16_t)(t_pack2<F16, ES, CONV>(v[k], 0u) & 0xFFFFu));
     }
   }
 }
@@ -370,7 +383,7 @@ KK_DQ_DEV void codebook8(float scale, uint32_t x0, uint32_t x1, float (&y)[8]) {
   for (int e = 0; e < 8; ++e) y[e] = __fmul_rn(scale, byte_to_float<128>(e < 4 ? r0 : r1, e & 3));
 }
 // 32-weight codebook blocks: lane l takes elements 8(l&3)..+8 of block (l>>2), eight blocks per warp iteration (as consume_legacy32).
-template <uint32_t BYTES, int TABLE>
+template <bool F16, uint32_t BYTES, int TABLE>
 KK_DQ_DEV void consume_codebook32(const Dsts& D, uint32_t pay, uint32_t nblk, uint64_t dst_off, int cwarp, int lane) {
   constexpr uint32_t kQsOff = BYTES - 16u;  // 2 (fp16 d) or 1 (E8M0 byte)
   const uint32_t e0 = 8u * (uint32_t)(lane & 3);
@@ -394,11 +407,12 @@ KK_DQ_DEV void consume_codebook32(const Dsts& D, uint32_t pay, uint32_t nblk, ui
       q1 = (q1 >> nsh) & 0x0F0F0F0Fu;
       float y[8];
       codebook8<TABLE>(d, q0, q1, y);
-      if (b < nblk) store_bf16x8(D, dst_off + (uint64_t)b * 64u + (uint32_t)(lane & 3) * 16u, y);
+      if (b < nblk) store_out8<F16>(D, dst_off + (uint64_t)b * 64u + (uint32_t)(lane & 3) * 16u, y);
     }
   }
 }
 // IQ4_XS: lane l handles elements 8l..8l+7 = sub-block j = l>>2, i = 8(l&3)..+8; one super-block per warp iteration.
+template <bool F16>
 KK_DQ_DEV void consume_iq4xs(const Dsts& D, uint32_t pay, uint32_t nblk, uint64_t dst_off, int cwarp, int lane) {
   const uint32_t j = (uint32_t)(lane >> 2), i0 = 8u * (uint32_t)(lane & 3);
   const uint32_t q_off = 8u + 16u * j + (i0 & 15u);
@@ -415,7 +429,7 @@ KK_DQ_DEV void consume_iq4xs(const Dsts& D, uint32_t pay, uint32_t nblk, uint64_
     const uint32_t q1 = (lds32_blk<KK_IQ4XS_BLOCK_BYTES>(blk + q_off + 4u) >> nsh) & 0x0F0F0F0Fu;
     float y[8];
     codebook8<0>(dl, q0, q1, y);
-    store_bf16x8(D, dst_off + (uint64_t)b * 512u + (uint32_t)lane * 16u, y);
+    store_out8<F16>(D, dst_off + (uint64_t)b * 512u + (uint32_t)lane * 16u, y);
   }
 }
 
@@ -427,16 +441,18 @@ KK_DQ_DEV uint32_t ksigns7(uint32_t i7) { return i7 | ((kk_popc(i7) & 1u) << 7);
 KK_DQ_DEV float signed_mul(float db, uint32_t w, int k, uint32_t signs, int bit) {
   return kk_bits2f(kk_f2bits(__fmul_rn(db, byte_to_float<0>(w, k))) ^ (((signs >> bit) & 1u) << 31));
 }
+template <bool F16>
 KK_DQ_DEV void store_entry(const Dsts& D, uint64_t off, float db, uint32_t lo, uint32_t hi, uint32_t signs) {
   float y[8];
 #pragma unroll
   for (int e = 0; e < 8; ++e) y[e] = signed_mul(db, e < 4 ? lo : hi, e & 3, signs, e);
-  store_bf16x8(D, off, y);
+  store_out8<F16>(D, off, y);
 }
 // db = (d * (0.5 + s)) * K — two roundings, like gguf-py (K is a power of two, the second product is exact)
 KK_DQ_DEV float iq_scale(float d, uint32_t s, float k) { return __fmul_rn(__fmul_rn(d, __fadd_rn(0.5f, (float)s)), k); }
 
 // IQ2_XXS (66 B): d f16 | 8 x { u32: four grid indices (bytes) | u32: four 7-bit sign indices, scale in the top 4 bits }
+template <bool F16>
 KK_DQ_DEV void consume_iq2xxs(const Dsts& D, uint32_t pay, uint32_t nblk, uint64_t dst_off, int cwarp, int lane) {
   const uint32_t g = (uint32_t)(lane >> 2), k = (uint32_t)(lane & 3);
 #pragma unroll 2
@@ -445,11 +461,12 @@ KK_DQ_DEV void consume_iq2xxs(const Dsts& D, uint32_t pay, uint32_t nblk, uint64
     const float d = lds_f16(blk);
     const uint32_t q1 = lds32_blk<KK_IQ2XXS_BLOCK_BYTES>(blk + 6u + 8u * g);
     const uint64_t grid = kk_grid_iq2xxs(lds8(blk + 2u + 8u * g + k));
-    store_entry(D, dst_off + (uint64_t)b * 512u + (uint32_t)lane * 16u, iq_scale(d, q1 >> 28, 0.25f), (uint32_t)grid, (uint32_t)(grid >> 32),
+    store_entry<F16>(D, dst_off + (uint64_t)b * 512u + (uint32_t)lane * 16u, iq_scale(d, q1 >> 28, 0.25f), (uint32_t)grid, (uint32_t)(grid >> 32),
                 ksigns7((q1 >> (7u * k)) & 0x7Fu));
   }
 }
 // IQ2_XS (74 B): d f16 | 32 x u16 { 9-bit grid index | 7-bit sign index } | scales[8] (a nibble per 16 weights)
+template <bool F16>
 KK_DQ_DEV void consume_iq2xs(const Dsts& D, uint32_t pay, uint32_t nblk, uint64_t dst_off, int cwarp, int lane) {
   const uint32_t l = (uint32_t)lane;
 #pragma unroll 2
@@ -459,10 +476,11 @@ KK_DQ_DEV void consume_iq2xs(const Dsts& D, uint32_t pay, uint32_t nblk, uint64_
     const uint32_t q = lds16_any(blk + 2u + 2u * l);
     const uint32_t s = (lds8(blk + 66u + (l >> 2)) >> (4u * ((l >> 1) & 1u))) & 0xFu;
     const uint64_t grid = kk_grid_iq2xs(q & 511u);
-    store_entry(D, dst_off + (uint64_t)b * 512u + l * 16u, iq_scale(d, s, 0.25f), (uint32_t)grid, (uint32_t)(grid >> 32), ksigns7(q >> 9));
+    store_entry<F16>(D, dst_off + (uint64_t)b * 512u + l * 16u, iq_scale(d, s, 0.25f), (uint32_t)grid, (uint32_t)(grid >> 32), ksigns7(q >> 9));
   }
 }
 // IQ2_S (82 B): d f16 | qs[32] | signs[32] | qh[8] (2 more index bits per entry) | scales[8]
+template <bool F16>
 KK_DQ_DEV void consume_iq2s(const Dsts& D, uint32_t pay, uint32_t nblk, uint64_t dst_off, int cwarp, int lane) {
   const uint32_t l = (uint32_t)lane;
   // (no `#pragma unroll 2` here: this loop is not latency-bound, and it ran slower unrolled)
@@ -472,10 +490,11 @@ KK_DQ_DEV void consume_iq2s(const Dsts& D, uint32_t pay, uint32_t nblk, uint64_t
     const uint32_t idx = lds8(blk + 2u + l) | (((lds8(blk + 66u + (l >> 2)) >> (2u * (l & 3u))) & 3u) << 8);
     const uint32_t s = (lds8(blk + 74u + (l >> 2)) >> (4u * ((l >> 1) & 1u))) & 0xFu;
     const uint64_t grid = kk_grid_iq2s(idx);
-    store_entry(D, dst_off + (uint64_t)b * 512u + l * 16u, iq_scale(d, s, 0.25f), (uint32_t)grid, (uint32_t)(grid >> 32), lds8(blk + 34u + l));
+    store_entry<F16>(D, dst_off + (uint64_t)b * 512u + l * 16u, iq_scale(d, s, 0.25f), (uint32_t)grid, (uint32_t)(grid >> 32), lds8(blk + 34u + l));
   }
 }
 // IQ3_XXS (98 B): d f16 | qs[64] (one 4-value entry per byte) | 8 x u32 { four 7-bit sign indices, scale in the top 4 bits }
+template <bool F16>
 KK_DQ_DEV void consume_iq3xxs(const Dsts& D, uint32_t pay, uint32_t nblk, uint64_t dst_off, int cwarp, int lane) {
   const uint32_t l = (uint32_t)lane, g = l >> 2, k = l & 3u;
 #pragma unroll 2
@@ -484,10 +503,11 @@ KK_DQ_DEV void consume_iq3xxs(const Dsts& D, uint32_t pay, uint32_t nblk, uint64
     const float d = lds_f16(blk);
     const uint32_t w = lds32_blk<KK_IQ3XXS_BLOCK_BYTES>(blk + 66u + 4u * g);
     const uint32_t lo = kk_grid_iq3xxs(lds8(blk + 2u + 2u * l)), hi = kk_grid_iq3xxs(lds8(blk + 3u + 2u * l));
-    store_entry(D, dst_off + (uint64_t)b * 512u + l * 16u, iq_scale(d, w >> 28, 0.5f), lo, hi, ksigns7((w >> (7u * k)) & 0x7Fu));
+    store_entry<F16>(D, dst_off + (uint64_t)b * 512u + l * 16u, iq_scale(d, w >> 28, 0.5f), lo, hi, ksigns7((w >> (7u * k)) & 0x7Fu));
   }
 }
 // IQ3_S (110 B): d f16 | qs[64] | qh[8] (a ninth index bit per entry) | signs[32] | scales[4] (a nibble per 32 weights); db = d * (1 + 2s)
+template <bool F16>
 KK_DQ_DEV void consume_iq3s(const Dsts& D, uint32_t pay, uint32_t nblk, uint64_t dst_off, int cwarp, int lane) {
   const uint32_t l = (uint32_t)lane, g = l >> 2;
 #pragma unroll 2
@@ -498,18 +518,20 @@ KK_DQ_DEV void consume_iq3s(const Dsts& D, uint32_t pay, uint32_t nblk, uint64_t
     const uint32_t i0 = lds8(blk + 2u + 2u * l) | (((qh >> ((2u * l) & 7u)) & 1u) << 8);
     const uint32_t i1 = lds8(blk + 3u + 2u * l) | (((qh >> (((2u * l) & 7u) + 1u)) & 1u) << 8);
     const uint32_t s = (lds8(blk + 106u + (g >> 1)) >> (4u * (g & 1u))) & 0xFu;
-    store_entry(D, dst_off + (uint64_t)b * 512u + l * 16u, __fmul_rn(d, (float)(1u + 2u * s)), kk_grid_iq3s(i0), kk_grid_iq3s(i1), lds8(blk + 74u + l));
+    store_entry<F16>(D, dst_off + (uint64_t)b * 512u + l * 16u, __fmul_rn(d, (float)(1u + 2u * s)), kk_grid_iq3s(i0), kk_grid_iq3s(i1), lds8(blk + 74u + l));
   }
 }
 // IQ1_S / IQ1_M: codebook values in {-1, 0, 1} (stored + 1), y = dl * (value + delta), delta = +-0.125
+template <bool F16>
 KK_DQ_DEV void store_entry_iq1(const Dsts& D, uint64_t off, float dl, uint64_t grid, float delta) {
   const uint32_t lo = (uint32_t)grid, hi = (uint32_t)(grid >> 32);
   float y[8];
 #pragma unroll
   for (int e = 0; e < 8; ++e) y[e] = __fmul_rn(dl, __fadd_rn(byte_to_float<1>(e < 4 ? lo : hi, e & 3), delta));
-  store_bf16x8(D, off, y);
+  store_out8<F16>(D, off, y);
 }
 // IQ1_S (50 B): d f16 | qs[32] | 8 x u16 { four 3-bit index extensions | 3-bit scale << 12 | delta sign << 15 }
+template <bool F16>
 KK_DQ_DEV void consume_iq1s(const Dsts& D, uint32_t pay, uint32_t nblk, uint64_t dst_off, int cwarp, int lane) {
   const uint32_t l = (uint32_t)lane, g = l >> 2, k = l & 3u;
 #pragma unroll 2
@@ -518,11 +540,12 @@ KK_DQ_DEV void consume_iq1s(const Dsts& D, uint32_t pay, uint32_t nblk, uint64_t
     const float d = lds_f16(blk);
     const uint32_t qh = lds16_any(blk + 34u + 2u * g);
     const uint32_t idx = lds8(blk + 2u + l) | (((qh >> (3u * k)) & 7u) << 8);
-    store_entry_iq1(D, dst_off + (uint64_t)b * 512u + l * 16u, __fmul_rn(d, (float)(2u * ((qh >> 12) & 7u) + 1u)), kk_grid_iq1s(idx),
+    store_entry_iq1<F16>(D, dst_off + (uint64_t)b * 512u + l * 16u, __fmul_rn(d, (float)(2u * ((qh >> 12) & 7u) + 1u)), kk_grid_iq1s(idx),
                     (qh & 0x8000u) ? -0.125f : 0.125f);
   }
 }
 // IQ1_M (56 B): qs[32] | qh[16] (a nibble per entry: 3 index bits, bit 3 = delta sign) | 4 x u16 { four 3-bit scales | a nibble of the fp16 d }
+template <bool F16>
 KK_DQ_DEV void consume_iq1m(const Dsts& D, uint32_t pay, uint32_t nblk, uint64_t dst_off, int cwarp, int lane) {
   const uint32_t l = (uint32_t)lane, k16 = l >> 1;
 #pragma unroll 2
@@ -533,11 +556,12 @@ KK_DQ_DEV void consume_iq1m(const Dsts& D, uint32_t pay, uint32_t nblk, uint64_t
     const uint32_t sw = (k16 >> 2) == 0 ? s0 : (k16 >> 2) == 1 ? s1 : (k16 >> 2) == 2 ? s2 : s3;
     const uint32_t sc = (sw >> (3u * (k16 & 3u))) & 7u;
     const uint32_t nib = (lds8(blk + 32u + (l >> 1)) >> (4u * (l & 1u))) & 0xFu;
-    store_entry_iq1(D, dst_off + (uint64_t)b * 512u + l * 16u, __fmul_rn(d, (float)(2u * sc + 1u)), kk_grid_iq1s(lds8(blk + l) | ((nib & 7u) << 8)),
+    store_entry_iq1<F16>(D, dst_off + (uint64_t)b * 512u + l * 16u, __fmul_rn(d, (float)(2u * sc + 1u)), kk_grid_iq1s(lds8(blk + l) | ((nib & 7u) << 8)),
                     (nib & 8u) ? -0.125f : 0.125f);
   }
 }
 // TQ2_0 (66 B): qs[64] | d f16; weight 128h + 32s + i = ((qs[32h+i] >> 2s) & 3) - 1 — Q2_K's bit layout without scales
+template <bool F16>
 KK_DQ_DEV void consume_tq2_0(const Dsts& D, uint32_t pay, uint32_t nblk, uint64_t dst_off, int cwarp, int lane) {
   const uint32_t q_off = 32u * (uint32_t)(lane >> 4) + 8u * (uint32_t)(lane & 3);
   const uint32_t sh = 2u * (uint32_t)((lane >> 2) & 3);
@@ -549,7 +573,7 @@ KK_DQ_DEV void consume_tq2_0(const Dsts& D, uint32_t pay, uint32_t nblk, uint64_
     float y[8];
 #pragma unroll
     for (int e = 0; e < 8; ++e) y[e] = __fmul_rn(d, byte_to_float<1>(e < 4 ? q0 : q1, e & 3));
-    store_bf16x8(D, dst_off + (uint64_t)b * 512u + (uint32_t)lane * 16u, y);
+    store_out8<F16>(D, dst_off + (uint64_t)b * 512u + (uint32_t)lane * 16u, y);
   }
 }
 // TQ1_0 (54 B): qs[48] | qh[4] | d f16 — base-3 digits: trit = (((B * 3^p) & 255) * 3) >> 8.  Four source bytes are processed as two
@@ -559,6 +583,7 @@ KK_DQ_DEV uint32_t tq1_trits4(uint32_t w, uint32_t m) {
   const uint32_t od = (((((w >> 8) & 0x00FF00FFu) * m) & 0x00FF00FFu) * 3u >> 8) & 0x00030003u;  // bytes 1 and 3
   return ev | (od << 8);
 }
+template <bool F16>
 KK_DQ_DEV void consume_tq1_0(const Dsts& D, uint32_t pay, uint32_t nblk, uint64_t dst_off, int cwarp, int lane) {
   // weights 8l..8l+7: lanes 0-19 read qs[0..31] with power l/4, lanes 20-29 qs[32..47] with power (l-20)/2, lanes 30-31 all of qh with
   // powers 2(l-30) (first four weights) and 2(l-30)+1 (last four)
@@ -576,12 +601,13 @@ KK_DQ_DEV void consume_tq1_0(const Dsts& D, uint32_t pay, uint32_t nblk, uint64_
     float y[8];
 #pragma unroll
     for (int e = 0; e < 8; ++e) y[e] = __fmul_rn(d, byte_to_float<1>(e < 4 ? t0 : t1, e & 3));
-    store_bf16x8(D, dst_off + (uint64_t)b * 512u + l * 16u, y);
+    store_out8<F16>(D, dst_off + (uint64_t)b * 512u + l * 16u, y);
   }
 }
 // NVFP4 (36 B, 64 weights): 4 x UE4M3 scale (one per 16 weights) | qs[32]; sub-block s uses qs[8s..8s+7]: low nibbles = its first 8 weights,
 // high nibbles the next 8; y = (scale / 2) * kMXFP4[q4] (doubled e2m1 table).  Lane l: block l>>3 of four per warp iteration, sub-block (l>>1)&3,
 // half l&1.
+template <bool F16>
 KK_DQ_DEV void consume_nvfp4(const Dsts& D, uint32_t pay, uint32_t nblk, uint64_t dst_off, int cwarp, int lane) {
   const uint32_t l = (uint32_t)lane, sb = (l >> 1) & 3u, nsh = 4u * (l & 1u);
 #pragma unroll 2
@@ -596,7 +622,7 @@ KK_DQ_DEV void consume_nvfp4(const Dsts& D, uint32_t pay, uint32_t nblk, uint64_
       const uint32_t q0 = (lds32_blk<KK_NVFP4_BLOCK_BYTES>(blk + 4u + 8u * sb) >> nsh) & 0x0F0F0F0Fu, q1 = (lds32_blk<KK_NVFP4_BLOCK_BYTES>(blk + 8u + 8u * sb) >> nsh) & 0x0F0F0F0Fu;
       float y[8];
       codebook8<1>(d, q0, q1, y);
-      if (b < nblk) store_bf16x8(D, dst_off + (uint64_t)b * 128u + (l & 7u) * 16u, y);
+      if (b < nblk) store_out8<F16>(D, dst_off + (uint64_t)b * 128u + (l & 7u) * 16u, y);
     }
   }
 }

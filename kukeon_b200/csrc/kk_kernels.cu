@@ -18,6 +18,10 @@
 //   broadcast are ONE kernel and the source bytes are read from HBM exactly once.
 //   The kernel keeps the tile scheduling and the stage protocol; the segment lookup (kk_tile_seg), the tile (kk_make_tile), its copies
 //   (kk_load_tile), its bulk stores (kk_store_tile) and the consumer dispatch (kk_consume_tile) are the functions tests/emul plays on the CPU.
+//
+// kk_convert_f16_kernel: the same kernel instantiated for IEEE fp16 output (KK_LOAD_F16 models; launch_convert picks it from
+//   KK_LAUNCH_F16).  Every pack is cvt.rn.f16x2.f32 instead of cvt.rn.bf16x2.f32, the 16-bit casts take bf16 in, and FP8 stores the
+//   hardware's f16x2 pair as it is.  Two kernels rather than a branch: neither reads the flag, and the bf16 kernel's code is unchanged.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
@@ -121,6 +125,12 @@ __device__ __forceinline__ void bulk_load(const StageLoad& S, uint32_t stage_off
 __device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
   uint32_t r;
   asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(b), "f"(a));
+  return r;
+}
+// Two floats -> packed f16x2 (a in the low half), round-to-nearest-even, overflow -> +-inf, fp16 subnormals kept; NaN -> 0x7FFF.
+__device__ __forceinline__ uint32_t pack_f16x2(float a, float b) {
+  uint32_t r;
+  asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(b), "f"(a));
   return r;
 }
 
@@ -246,7 +256,9 @@ __device__ __forceinline__ KKSeg load_seg(const KKSeg* p) {
   return s;
 }
 
-__global__ void __launch_bounds__(kThreads, 1) kk_convert_kernel(const ConvertLaunch L) {
+// The kernel body, for either output format (F16: KK_LAUNCH_F16); the two __global__ instantiations follow it.
+template <bool F16>
+__device__ __forceinline__ void convert_body(const ConvertLaunch& L) {
   extern __shared__ __align__(128) uint8_t smem[];
   uint8_t* stage_buf = smem;
   TileDesc* descs = reinterpret_cast<TileDesc*>(smem + kStages * kStageBytes);
@@ -375,7 +387,7 @@ __global__ void __launch_bounds__(kThreads, 1) kk_convert_kernel(const ConvertLa
         mbar_arrive(empty0 + 8 * pending);
         pending = -1;
       }
-      kk_consume_tile(D, t, sbase, pay, L, cwarp, lane, ctid, it);
+      kk_consume_tile<F16>(D, t, sbase, pay, L, cwarp, lane, ctid, it);
       __syncwarp();
       if (lane == 0) mbar_arrive(empty0 + 8 * s);
     }
@@ -388,6 +400,10 @@ __global__ void __launch_bounds__(kThreads, 1) kk_convert_kernel(const ConvertLa
     }
   }
 }
+
+__global__ void __launch_bounds__(kThreads, 1) kk_convert_kernel(const ConvertLaunch L) { convert_body<false>(L); }
+// fp16 output.  Its name must not contain "kk_convert_kernel": tools/sass_budget.py finds the bf16 kernel by that substring.
+__global__ void __launch_bounds__(kThreads, 1) kk_convert_f16_kernel(const ConvertLaunch L) { convert_body<true>(L); }
 
 // ---- checksum ---------------------------------------------------------------------------------
 __device__ __forceinline__ uint64_t mix64(uint64_t x) {
@@ -435,7 +451,10 @@ __global__ void __launch_bounds__(256) kk_fill_kernel(uint4* __restrict__ dst, u
 }  // namespace
 
 cudaError_t kernels_init_device() {
-  return cudaFuncSetAttribute(kk_convert_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kSmemFixed + 4 * kMaxSegsPerLaunch + 128));
+  const int smem = (int)(kSmemFixed + 4 * kMaxSegsPerLaunch + 128);
+  const cudaError_t e = cudaFuncSetAttribute(kk_convert_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  if (e != cudaSuccess) return e;
+  return cudaFuncSetAttribute(kk_convert_f16_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
 }
 
 cudaError_t launch_convert(const ConvertLaunch& L, int sm_count, cudaStream_t stream) {
@@ -443,7 +462,8 @@ cudaError_t launch_convert(const ConvertLaunch& L, int sm_count, cudaStream_t st
   if (L.n_segs == 0 || L.n_segs > kMaxSegsPerLaunch || L.n_dst == 0 || L.n_dst > KK_MAX_DST || !L.sched) return cudaErrorInvalidValue;
   const uint32_t grid = L.n_tiles < (uint32_t)sm_count ? L.n_tiles : (uint32_t)sm_count;
   const size_t smem = kSmemFixed + 4 * (size_t)L.n_segs + 16;
-  kk_convert_kernel<<<grid, kThreads, smem, stream>>>(L);
+  if (L.flags & KK_LAUNCH_F16) kk_convert_f16_kernel<<<grid, kThreads, smem, stream>>>(L);
+  else kk_convert_kernel<<<grid, kThreads, smem, stream>>>(L);
   return cudaGetLastError();
 }
 

@@ -186,11 +186,14 @@ bool part_pool_range(const Plan& P, int part, uint64_t& lo, uint64_t& hi) {
   return linear;
 }
 
-// Destination pools a convert launch on local device `li` writes to.
+// The output format of m's convert launches: KK_LAUNCH_F16 for a KK_LOAD_F16 model, which launch_convert runs on the fp16 kernel.
+uint32_t format_flags(const kk_model* m) { return (m->plan.flags & KK_LOAD_F16) ? KK_LAUNCH_F16 : 0u; }
+
+// Destination pools a convert launch on local device `li` writes to, and the launch's output format.
 void fill_dsts(kk_model* m, int li, ConvertLaunch& L) {
   const LoadShape& S = m->shape;
   L.n_dst = 0;
-  L.flags = 0;
+  L.flags = format_flags(m);
   for (auto& d : L.dst) d = nullptr;
   L.dst[L.n_dst++] = m->pools[(size_t)li].ptr;
   L.n_xdst = 0;
@@ -233,7 +236,7 @@ void fill_dsts(kk_model* m, int li, ConvertLaunch& L) {
 // Peer raw images a stage-1 copy launch on local device li writes to (never the local image: it is the source).
 void fill_raw_dsts(kk_model* m, int li, ConvertLaunch& L) {
   L.n_dst = 0;
-  L.flags = 0;
+  L.flags = format_flags(m);
   for (auto& d : L.dst) d = nullptr;
   if (m->shape.multi_proc) {
     for (auto& b : m->peer[kPeerRaw])
@@ -457,6 +460,7 @@ void convert_local_all(kk_model* m, float* ms_total) {
   for (size_t li = 0; li < launches.size(); ++li) {
     ConvertLaunch base{};
     base.n_dst = 1;
+    base.flags = format_flags(m);
     base.dst[0] = m->pools[li].ptr;
     launches[li] = image_launches(base, m->images[li]);
   }
@@ -507,6 +511,7 @@ void pull_slices(kk_model* m, float* ms_total) {
     L.n_segs = (uint32_t)segs.size();
     L.n_tiles = (uint32_t)tiles;
     L.n_dst = 1;
+    L.flags = format_flags(m);
     L.dst[0] = m->pools[0].ptr;
     launches[0].push_back(L);
   }

@@ -69,6 +69,12 @@
 #define KK_MAX_DST 8
 /* ConvertLaunch::flags */
 #define KK_LAUNCH_MULTIMEM 0x2u       /* dst[0] is an NVLS multicast address: store with multimem.st */
+#define KK_LAUNCH_F16 0x4u            /* IEEE fp16 output (a KK_LOAD_F16 model): launch_convert runs kk_convert_f16_kernel, the consumer bodies'
+                                         fp16 instantiation.  Op codes keep their numbers and _BF16 names, which name the default output; the
+                                         launch's format decides the actual one.  The two 16-bit casts (KK_OP_F16_BF16, KK_OP_T_F16_BF16) convert
+                                         FROM the 16-bit float that is not the output format: fp16 -> bf16 in a bf16 launch, bf16 -> fp16 in an
+                                         f16 launch.  Both formats are 2 bytes, so the geometry below, kk_make_tile, kk_seg_tiles and the producer
+                                         do not depend on the flag. */
 
 enum KKOp : uint32_t {
   KK_OP_COPY = 0,      // units = bytes

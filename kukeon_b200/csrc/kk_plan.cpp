@@ -26,23 +26,29 @@ struct OpInfo {
   uint64_t tile_units;      // op units per tile (split granule)
 };
 
-// op for a non-transposed tensor of file dtype dt.
+// op for a non-transposed tensor of file dtype dt.  Every float output is bf16, or fp16 under KK_LOAD_F16 (out): the op codes are the
+// same, the launch's output format (KK_LAUNCH_F16) picks the kernel.  Under it the 16-bit roles swap: F16 is the verbatim copy and BF16
+// takes the 16-bit cast.
 OpInfo op_for(uint32_t dt, uint32_t flags, const std::string& name) {
+  const bool f16 = (flags & KK_LOAD_F16) != 0;
+  const uint32_t out = f16 ? KK_F16 : KK_BF16;
   switch (dt) {
-    case KK_BF16: return {KK_OP_COPY, KK_BF16, 1, 1, KK_TILE_SRC_BYTES};
+    case KK_BF16:
+    case KK_F16:
+      if (dt == out) return {KK_OP_COPY, out, 1, 1, KK_TILE_SRC_BYTES};
+      return {KK_OP_F16_BF16, out, 2, 2, KK_TILE_SRC_BYTES / 2};
     case KK_F32:
       if (flags & KK_LOAD_KEEP_F32) return {KK_OP_COPY, KK_F32, 1, 1, KK_TILE_SRC_BYTES};
-      return {KK_OP_F32_BF16, KK_BF16, 4, 2, KK_TILE_SRC_BYTES / 4};
-    case KK_F16: return {KK_OP_F16_BF16, KK_BF16, 2, 2, KK_TILE_SRC_BYTES / 2};
+      return {KK_OP_F32_BF16, out, 4, 2, KK_TILE_SRC_BYTES / 4};
     case KK_F8_E4M3:
-      if (flags & KK_LOAD_F8_TO_BF16) return {KK_OP_F8E4M3_BF16, KK_BF16, 1, 2, KK_TILE_SRC_BYTES};
+      if (flags & KK_LOAD_F8_TO_BF16) return {KK_OP_F8E4M3_BF16, out, 1, 2, KK_TILE_SRC_BYTES};
       break;
     case KK_F8_E5M2:
-      if (flags & KK_LOAD_F8_TO_BF16) return {KK_OP_F8E5M2_BF16, KK_BF16, 1, 2, KK_TILE_SRC_BYTES};
+      if (flags & KK_LOAD_F8_TO_BF16) return {KK_OP_F8E5M2_BF16, out, 1, 2, KK_TILE_SRC_BYTES};
       break;
     default: break;
   }
-  // block-quantised GGUF types -> bf16 (geometry shared with the kernel: kk_ops.h)
+  // block-quantised GGUF types -> bf16 / fp16 (geometry shared with the kernel: kk_ops.h)
   uint32_t qop = KK_OP_COUNT;
   switch (dt) {
     case KK_Q4_0: qop = KK_OP_Q4_0_BF16; break;
@@ -72,7 +78,7 @@ OpInfo op_for(uint32_t dt, uint32_t flags, const std::string& name) {
   }
   if (qop != KK_OP_COUNT) {
     const KKBlockGeom g = kk_block_geom(qop);
-    return {qop, KK_BF16, g.block_bytes, g.out_bytes, g.tile_blocks};
+    return {qop, out, g.block_bytes, g.out_bytes, g.tile_blocks};
   }
   const DtypeInfo* di = dtype_info(dt);
   if (!di) fail(KK_EINVAL, "tensor %s: unknown dtype %u", name.c_str(), dt);
@@ -394,8 +400,9 @@ Plan build_plan(Index index, int mode, uint32_t flags, int n_parts, uint64_t chu
         if (R > 0xFFFFFFFFull || C > 0xFFFFFFFFull) fail(KK_EUNSUPPORTED, "tensor %s too large to transpose", t.name.c_str());
         uint32_t op, pdt;
         uint64_t es, oes;
-        if (t.dtype == KK_F32 && !(flags & KK_LOAD_KEEP_F32)) { op = KK_OP_T_F32_BF16; pdt = KK_BF16; es = 4; oes = 2; }
-        else if (t.dtype == KK_F16) { op = KK_OP_T_F16_BF16; pdt = KK_BF16; es = 2; oes = 2; }
+        const uint32_t out = (flags & KK_LOAD_F16) ? KK_F16 : KK_BF16;  // the float output format, as in op_for
+        if (t.dtype == KK_F32 && !(flags & KK_LOAD_KEEP_F32)) { op = KK_OP_T_F32_BF16; pdt = out; es = 4; oes = 2; }
+        else if ((t.dtype == KK_F16 || t.dtype == KK_BF16) && t.dtype != out) { op = KK_OP_T_F16_BF16; pdt = out; es = 2; oes = 2; }
         else if (t.dtype == KK_F32 || t.dtype == KK_I32 || t.dtype == KK_U32) { op = KK_OP_T_B32; pdt = t.dtype; es = 4; oes = 4; }
         else { op = KK_OP_T_B16; pdt = t.dtype; es = 2; oes = 2; }
         pc.oi = {op, pdt, es, oes, KK_T_ROWS};

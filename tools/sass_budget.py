@@ -10,7 +10,10 @@ issue-bound however well the memory side is arranged.
 A static count is an upper estimate of what issues (predicated-off instructions count; code behind a forward branch that is not taken
 counts) and knows nothing about stalls; it ranks the loops and says where the PRMT/FADD rewrites landed, it is not a measurement.
 
-    python tools/sass_budget.py [--md sass_budget.md] [--json sass_budget.json]
+    python tools/sass_budget.py [--kernel kk_convert_f16_kernel] [--md sass_budget.md] [--json sass_budget.json]
+
+--kernel names the kernel (a substring of its symbol): kk_convert_kernel, the bf16 kernel, by default; kk_convert_f16_kernel is the same
+source instantiated for fp16 output (KK_LOAD_F16 models).
 """
 import argparse
 import collections
@@ -63,7 +66,9 @@ def fresh_object():
     return obj if all(os.path.getmtime(x) <= os.path.getmtime(obj) for x in deps) else None
 
 
-def disassemble(obj=None):
+def disassemble(obj=None, resources=False):
+    """nvdisasm -gi text of the kernels' object; with resources=True also {symbol: {"REG": n, "STACK": n, "LOCAL": n, ...}} from
+    cuobjdump -res-usage of the same object."""
     with tempfile.TemporaryDirectory() as d:
         obj = obj or fresh_object()
         if obj is None:
@@ -72,14 +77,25 @@ def disassemble(obj=None):
                                    "-c", KERNEL_CU, "-o", obj], cwd=CSRC, stderr=subprocess.DEVNULL)
         subprocess.check_call(["cuobjdump", "-xelf", "all", obj], cwd=d, stdout=subprocess.DEVNULL)
         cubin = [f for f in os.listdir(d) if f.endswith(".cubin")][0]
-        return subprocess.check_output(["nvdisasm", "-gi", "-c", os.path.join(d, cubin)], text=True)
+        text = subprocess.check_output(["nvdisasm", "-gi", "-c", os.path.join(d, cubin)], text=True)
+        if not resources:
+            return text
+        res, fn = {}, None
+        for l in subprocess.check_output(["cuobjdump", "-res-usage", obj], text=True).split("\n"):
+            m = re.match(r"\s*Function (\S+):", l)
+            if m:
+                fn = m.group(1)
+            elif fn and "REG:" in l:
+                res[fn] = {k: int(v) for k, v in re.findall(r"(\w+):(\d+)", l)}
+                fn = None
+        return text, res
 
 
-def parse(text):
-    """-> list of dicts for the instructions of kk_convert_kernel: idx, op (mnemonic), chain (the inline frames (file, line, inlined-at file,
-    inlined-at line), innermost first), label index map."""
+def parse(text, kernel="kk_convert_kernel"):
+    """-> list of dicts for the instructions of `kernel` (a substring of its symbol): idx, op (mnemonic), chain (the inline frames (file,
+    line, inlined-at file, inlined-at line), innermost first), label index map."""
     lines = text.split("\n")
-    start = next(i for i, l in enumerate(lines) if l.startswith(".text.") and "kk_convert_kernel" in l)
+    start = next(i for i, l in enumerate(lines) if l.startswith(".text.") and kernel in l)
     ins, labels = [], {}
     chain, fresh = [], True
     ann = re.compile(r'//## File "([^"]+)", line (\d+)(?: inlined at "([^"]+)", line (\d+))?')
@@ -193,8 +209,9 @@ def classify(mn):
     return "other"
 
 
-def analyse():
-    ins, labels = parse(disassemble())
+def analyse(kernel="kk_convert_kernel", text=None):
+    """Per-op rows, total instructions and opcode counts of `kernel`; text: nvdisasm output to read (default: disassemble())."""
+    ins, labels = parse(text if text is not None else disassemble(), kernel)
     disp = dispatch_lines()
     owner = [dispatch_op(x["chain"], disp) for x in ins]
     loops = loops_of(ins, labels)
@@ -224,14 +241,15 @@ def analyse():
 
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--kernel", default="kk_convert_kernel", help="substring of the kernel's symbol (kk_convert_f16_kernel: the fp16-output kernel)")
     ap.add_argument("--md")
     ap.add_argument("--json", help="write {op: {hot, bytes_in, bytes_out, issue_ceiling_GBps}} (read by tools/gpu_quick_types.py to print prediction next to measurement)")
     args = ap.parse_args()
-    rows, total, _ = analyse()
+    rows, total, _ = analyse(args.kernel)
     issue_rate = SM_COUNT * SM_GHZ * ISSUE_PER_CLK  # G warp instructions / s
     names = [c for c, _ in CLASSES] + ["other"]
     out = []
-    out.append(f"kk_convert_kernel: {total} SASS instructions; issue rate {issue_rate:.0f} G warp-instr/s ({SM_COUNT} SMs x {SM_GHZ} GHz x {ISSUE_PER_CLK}/clk); "
+    out.append(f"{args.kernel}: {total} SASS instructions; issue rate {issue_rate:.0f} G warp-instr/s ({SM_COUNT} SMs x {SM_GHZ} GHz x {ISSUE_PER_CLK}/clk); "
                f"HBM copy peak {HBM_PEAK_GBS:.0f} GB/s\n")
     hdr = ["op", "SASS instr (whole op)", "main loop (static)", "hot path instr / warp iteration", "bytes in + out / iteration", "hot instr / KiB of traffic",
            "issue ceiling GB/s", "ceiling / HBM peak"] + names
