@@ -34,6 +34,7 @@ var modelOptionFlags = map[string]uint32{
 	"keepF32":             gpupool.FlagKeepF32,
 	"f8ToBf16":            gpupool.FlagF8ToBF16,
 	"f16":                 gpupool.FlagF16,
+	"hfLayout":            gpupool.FlagHFLayout,
 }
 
 // validateModels normalises and checks the models[] of one container.

@@ -38,6 +38,9 @@ const (
 	// FlagF16 stores every float output as IEEE fp16 instead of bf16 (F16 tensors verbatim, BF16 / F32 / GGUF blocks rounded once);
 	// the pool layout is that of the same load without it.  An f16 and a bf16 load of one file are two models.
 	FlagF16 uint32 = C.KK_LOAD_F16
+	// FlagHFLayout loads a GGUF checkpoint in Hugging Face layout: HF tensor names, one tensor per expert and llama's Q/K rows
+	// un-permuted.  GGUF only (llama, qwen2, qwen3).
+	FlagHFLayout uint32 = C.KK_LOAD_HF_LAYOUT
 )
 
 type Config struct {

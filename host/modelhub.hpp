@@ -56,6 +56,7 @@ constexpr uint32_t kFlagGPT2Conv1DTranspose = KK_LOAD_GPT2_CONV1D_T;
 constexpr uint32_t kFlagKeepF32 = KK_LOAD_KEEP_F32;
 constexpr uint32_t kFlagF8ToBF16 = KK_LOAD_F8_TO_BF16;
 constexpr uint32_t kFlagF16 = KK_LOAD_F16;  // every float output as IEEE fp16 instead of bf16, same pool layout
+constexpr uint32_t kFlagHFLayout = KK_LOAD_HF_LAYOUT;  // GGUF in Hugging Face layout: HF names, one tensor per expert, Q/K rows un-permuted
 
 struct Config {
   std::vector<int> devices{0};

@@ -135,6 +135,33 @@ typedef enum kk_fanout {
                                       for byte, so under this flag an F16 checkpoint's row-parallel tensors use the exchange and a BF16
                                       checkpoint's are gathered (as F32 tensors are).  Flags are part of a model's identity: an f16 and a bf16
                                       load of one file are two models. */
+#define KK_LOAD_HF_LAYOUT 0x100u    /* GGUF checkpoints only: load the checkpoint in Hugging Face layout, as transformers' safetensors files have it.
+                                      The load sees the HF view of the file before it plans, and every other flag, mode, fan-out, DEFER, parts,
+                                      pipeline stage (over the HF names) and VMM pools apply to that view unchanged.  Placements, kk_model_tensor,
+                                      kk_model_get_info and the manifest speak HF names and shapes only (a GGUF name is KK_ENOENT); the manifest
+                                      and kk_plan_describe add "layout":"hf" and "architecture".
+                                        names        token_embd -> model.embed_tokens, output_norm -> model.norm, output -> lm_head,
+                                                     blk.N.attn_norm -> model.layers.N.input_layernorm, blk.N.ffn_norm -> .post_attention_layernorm,
+                                                     blk.N.attn_{q,k,v} -> .self_attn.{q,k,v}_proj, blk.N.attn_output -> .self_attn.o_proj,
+                                                     blk.N.attn_{q,k}_norm -> .self_attn.{q,k}_norm (qwen3), blk.N.ffn_{gate,up,down} ->
+                                                     .mlp.{gate,up,down}_proj, blk.N.ffn_gate_inp -> .block_sparse_moe.gate (llama); each keeps
+                                                     its .weight / .bias; rope_freqs.weight keeps its name (HF engines compute it from the config)
+                                        experts      (llama) blk.N.ffn_{gate,up,down}_exps.weight [E, r, c] -> E tensors
+                                                     model.layers.N.block_sparse_moe.experts.e.{w1,w3,w2}.weight [r, c], expert e being bytes
+                                                     [e * nbytes / E, (e + 1) * nbytes / E) of the stack
+                                        Q / K rows   (llama: Llama, Mistral, Mixtral) llama.cpp's converter interleaves the two rotary halves of
+                                                     every head of q_proj / k_proj (weight and bias); the load un-permutes them while staging:
+                                                     HF row h*hd + k*hd/2 + i is file row h*hd + 2i + k, with head count
+                                                     <arch>.attention.head_count for q and .head_count_kv (default: head_count) for k and
+                                                     hd = rows / heads.  qwen2 / qwen3 use NEOX rotary and are not permuted.
+                                      Architectures (general.architecture): llama, qwen2, qwen3; any other is KK_EUNSUPPORTED, and so is any
+                                      tensor the table does not map (nothing is dropped).  KK_EINVAL on a safetensors checkpoint; KK_EFORMAT
+                                      when a needed metadata key is missing or ill-typed (integers: any GGUF integer type in 1..65535; a
+                                      per-layer array is KK_EUNSUPPORTED) or Q/K rows are not a multiple of 2 * heads; KK_EUNSUPPORTED when a
+                                      Q/K row is not whole blocks of its type (a 1-D block-quantised bias) or a Q/K (head, half) row group would
+                                      start off a 16-byte pool boundary.  Split GGUFs: the keys are the first shard's; a later shard that repeats
+                                      one must agree (KK_EFORMAT).  All are raised before any device
+                                      is touched.  Costs: Q/K rows are read one row per read and stage as (head, half) pieces. */
 
 typedef struct kk_ctx kk_ctx;     /* one per process (kukeond lifetime) */
 typedef struct kk_model kk_model; /* refcounted; one per (checkpoint identity, mode, flags, layer range) */

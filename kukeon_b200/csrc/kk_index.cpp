@@ -307,9 +307,49 @@ void gguf_skip_value(Cursor& c, uint32_t vt, int depth) {
   if (!sz) fail(KK_EFORMAT, "%s: GGUF unknown value type %u", c.file.c_str(), vt);
   c.skip(sz);
 }
+
+// Reads the value of metadata key `key` (type vt) into a GgufKey: a string, or an integer of any GGUF integer type in 1..65535.  A value
+// of another type is recorded as unusable, not refused: only a load that needs it fails.  A malformed value is refused like any other.
+GgufKey gguf_read_key(Cursor& c, const std::string& key, uint32_t vt, bool string) {
+  GgufKey k;
+  k.seen = true;
+  char why[160];
+  if (string && vt == 8) {
+    k.s = c.str();
+    return k;
+  }
+  if (!string && vt <= 11 && vt != 6 && vt != 7 && vt != 8 && vt != 9) {
+    const bool sgn = vt == 1 || vt == 3 || vt == 5 || vt == 11;
+    const uint64_t sz = gguf_scalar_size(vt);
+    c.need(sz);
+    uint64_t raw = 0;
+    memcpy(&raw, c.p + c.off, (size_t)sz);  // little-endian
+    c.off += sz;
+    int64_t v = (int64_t)raw;
+    if (sgn && sz < 8 && (raw >> (sz * 8 - 1)) & 1) v = (int64_t)(raw | (~0ull << (sz * 8)));  // sign-extend
+    if ((sgn && v < 1) || (!sgn && raw < 1) || (sgn ? (uint64_t)v : raw) > 65535) {
+      snprintf(why, sizeof why, "%s = %lld is out of range 1..65535", key.c_str(), sgn ? (long long)v : (long long)std::min<uint64_t>(raw, INT64_MAX));
+      k.err = KK_EFORMAT;
+      k.why = why;
+    } else {
+      k.u = sgn ? (uint64_t)v : raw;
+    }
+    return k;
+  }
+  gguf_skip_value(c, vt, 0);
+  if (!string && vt == 9) {
+    snprintf(why, sizeof why, "%s is a per-layer array, which is not supported", key.c_str());
+    k.err = KK_EUNSUPPORTED;
+  } else {
+    snprintf(why, sizeof why, "%s has GGUF value type %u, not %s", key.c_str(), vt, string ? "a string" : "an integer");
+    k.err = KK_EFORMAT;
+  }
+  k.why = why;
+  return k;
+}
 }  // namespace
 
-void index_gguf_file(const std::string& file, uint32_t shard, std::vector<TensorRec>& out, uint64_t* file_bytes) {
+void index_gguf_file(const std::string& file, uint32_t shard, std::vector<TensorRec>& out, uint64_t* file_bytes, GgufMeta* meta) {
   MappedFile mf(file);
   if (file_bytes) *file_bytes = mf.n;
   Cursor c{mf.p, mf.n, 0, file};
@@ -324,6 +364,8 @@ void index_gguf_file(const std::string& file, uint32_t shard, std::vector<Tensor
   if (n_tensors > (1ull << 24) || n_kv > (1ull << 24)) fail(KK_EFORMAT, "%s: implausible GGUF counts", file.c_str());
   uint64_t alignment = 32;
   std::set<std::string> keys;
+  GgufMeta m;
+  std::map<std::string, GgufKey> per_arch;  // <any>.attention.head_count(_kv) / <any>.expert_count: general.architecture may come later
   for (uint64_t i = 0; i < n_kv; ++i) {
     std::string key = c.str();
     if (!keys.insert(key).second) fail(KK_EFORMAT, "%s: duplicate GGUF key %s", file.c_str(), key.c_str());
@@ -333,9 +375,25 @@ void index_gguf_file(const std::string& file, uint32_t shard, std::vector<Tensor
       alignment = c.get<uint32_t>();
       if (alignment == 0 || (alignment & (alignment - 1)) != 0)
         fail(KK_EFORMAT, "%s: invalid alignment: must be a non-zero power of two", file.c_str());
+    } else if (key == "general.architecture") {
+      m.arch = gguf_read_key(c, key, vt, true);
+    } else if (ends_with(key, ".attention.head_count") || ends_with(key, ".attention.head_count_kv") || ends_with(key, ".expert_count")) {
+      per_arch[key] = gguf_read_key(c, key, vt, false);
     } else {
       gguf_skip_value(c, vt, 0);
     }
+  }
+  if (meta) {
+    if (m.arch.seen && !m.arch.err) {
+      auto take = [&](const char* suffix, GgufKey& k) {
+        auto it = per_arch.find(m.arch.s + suffix);
+        if (it != per_arch.end()) k = it->second;
+      };
+      take(".attention.head_count", m.head_count);
+      take(".attention.head_count_kv", m.head_count_kv);
+      take(".expert_count", m.expert_count);
+    }
+    *meta = m;
   }
   struct Ent { TensorRec t; uint64_t rel; };
   std::vector<Ent> ents;
@@ -440,8 +498,23 @@ Index index_files(const std::string& dir, const std::vector<std::string>& names,
     uint32_t sid = (uint32_t)ix.shards.size();
     ix.shards.push_back(dir.empty() ? f : dir + "/" + f);
     uint64_t fb = 0;
-    if (gguf) index_gguf_file(ix.shards.back(), sid, ix.tensors, &fb);
-    else index_safetensors_file(ix.shards.back(), sid, ix.tensors, &fb);
+    if (gguf) {
+      GgufMeta m;
+      index_gguf_file(ix.shards.back(), sid, ix.tensors, &fb, &m);
+      if (sid == 0) ix.gguf = m;
+      else {  // the keys are the first shard's; a later shard that repeats one must agree, a disagreement is raised by a load that needs it
+        GgufKey* first[] = {&ix.gguf.arch, &ix.gguf.head_count, &ix.gguf.head_count_kv, &ix.gguf.expert_count};
+        const GgufKey* later[] = {&m.arch, &m.head_count, &m.head_count_kv, &m.expert_count};
+        for (int k = 0; k < 4; ++k)
+          if (later[k]->seen && first[k]->seen && !(*later[k] == *first[k]) && first[k]->err == 0) {
+            first[k]->seen = true;
+            first[k]->err = KK_EFORMAT;
+            first[k]->why = "shard " + ix.shards.back() + " disagrees with the first shard on a metadata key the HF layout reads";
+          }
+      }
+    } else {
+      index_safetensors_file(ix.shards.back(), sid, ix.tensors, &fb);
+    }
     ix.shard_bytes.push_back(fb);
   }
   sort_index(ix);

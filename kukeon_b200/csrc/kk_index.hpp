@@ -17,6 +17,8 @@ struct TensorRec {
   uint32_t shard = 0;
   uint64_t file_offset = 0;
   uint64_t nbytes = 0;
+  // to_hf_layout (kk_plan.hpp): llama.cpp interleaved the two rotary halves of each of this many heads in the rows (0: rows as in the file)
+  uint32_t rope_heads = 0;
   uint64_t n_elems() const {
     uint64_t n = 1;
     for (auto d : shape) n *= d;
@@ -24,8 +26,29 @@ struct TensorRec {
   }
 };
 
+// One GGUF metadata value, recorded as the file has it.  Indexing never fails on these: a load that needs the value (to_hf_layout)
+// raises err with why, or KK_EFORMAT when the key is missing.
+struct GgufKey {
+  bool seen = false;  // the key is in the file
+  int err = 0;        // seen: 0 when the value is usable, else KK_EFORMAT (ill-typed, out of range) or KK_EUNSUPPORTED (a per-layer array)
+  std::string why;
+  uint64_t u = 0;     // integer keys: 1..65535
+  std::string s;      // string keys
+  bool operator==(const GgufKey& o) const { return seen == o.seen && err == o.err && u == o.u && s == o.s; }
+};
+
+// The GGUF metadata the HF view (KK_LOAD_HF_LAYOUT) reads.  <arch> is general.architecture.
+struct GgufMeta {
+  GgufKey arch;           // general.architecture
+  GgufKey head_count;     // <arch>.attention.head_count
+  GgufKey head_count_kv;  // <arch>.attention.head_count_kv (absent for MHA models: then head_count)
+  GgufKey expert_count;   // <arch>.expert_count
+};
+
 struct Index {
   std::string format;               // "safetensors" | "gguf"
+  GgufMeta gguf;                    // GGUF: from the first shard (a later shard that repeats a key and disagrees marks it bad)
+  std::string hf_arch;              // to_hf_layout (kk_plan.hpp): the tensors are the HF view of a checkpoint of this architecture
   std::vector<std::string> shards;  // absolute paths
   std::vector<uint64_t> shard_bytes;
   std::vector<TensorRec> tensors;   // sorted by (shard, file_offset, name)
@@ -40,6 +63,6 @@ Index index_path(const std::string& path);
 
 // Exposed for tests of the individual parsers.
 void index_safetensors_file(const std::string& file, uint32_t shard, std::vector<TensorRec>& out, uint64_t* file_bytes);
-void index_gguf_file(const std::string& file, uint32_t shard, std::vector<TensorRec>& out, uint64_t* file_bytes);
+void index_gguf_file(const std::string& file, uint32_t shard, std::vector<TensorRec>& out, uint64_t* file_bytes, GgufMeta* meta = nullptr);
 
 }  // namespace kk

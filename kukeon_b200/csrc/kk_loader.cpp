@@ -787,7 +787,7 @@ kk_model* model_load(kk_ctx* c, const std::string& path, const kk_load_opts& opt
   const LoadShape& S = m->shape;
   try {
     double t0 = now_s();
-    Index ix = select_layers(index_path(path), opts.layer_begin, opts.layer_end);
+    Index ix = select_layers(to_hf_layout(index_path(path), opts.flags), opts.layer_begin, opts.layer_end);
     m->t_index = now_s() - t0;
     t0 = now_s();
     m->plan = build_plan(std::move(ix), opts.mode, opts.flags & ~KK_LOAD_DEFER, S.n_parts, c->slot_bytes);
@@ -1050,6 +1050,7 @@ static std::string build_manifest(kk_model* m, int li) {
     << "\",\"poolBytes\":" << m->pools[(size_t)li].bytes << ",\"mode\":" << m->plan.mode << ",\"format\":\"" << m->plan.index.format
     << "\",\"align\":" << KK_POOL_ALIGN;
   const Index& ix = m->plan.index;
+  if (!ix.hf_arch.empty()) o << ",\"layout\":\"hf\",\"architecture\":\"" << json_escape(ix.hf_arch) << "\"";
   if (ix.layer_end) o << ",\"layerBegin\":" << ix.layer_begin << ",\"layerEnd\":" << ix.layer_end << ",\"nLayers\":" << ix.n_layers;
   o << ",\"tensors\":[";
   for (size_t i = 0; i < T.size(); ++i) {

@@ -4,6 +4,7 @@
 
 #include <algorithm>
 #include <cstring>
+#include <set>
 #include <sstream>
 
 #include "kk_json.hpp"
@@ -365,6 +366,150 @@ Index select_layers(Index ix, uint32_t begin, uint32_t end) {
   return ix;
 }
 
+namespace {
+
+uint32_t need_key(const GgufKey& k, const char* key) {
+  if (!k.seen) fail(KK_EFORMAT, "KK_LOAD_HF_LAYOUT: the GGUF metadata has no %s", key);
+  if (k.err) fail(k.err, "KK_LOAD_HF_LAYOUT: %s", k.why.c_str());
+  return (uint32_t)k.u;
+}
+
+// The rename table, restated from gguf-py's tensor_mapping for llama / qwen2 / qwen3: per-layer GGUF base name -> HF name under
+// model.layers.N., and which architectures carry it.
+struct HfName { const char* gguf; const char* hf; bool llama, qwen2, qwen3; };
+const HfName kLayerNames[] = {
+    {"attn_norm", "input_layernorm", true, true, true},        {"ffn_norm", "post_attention_layernorm", true, true, true},
+    {"attn_q", "self_attn.q_proj", true, true, true},          {"attn_k", "self_attn.k_proj", true, true, true},
+    {"attn_v", "self_attn.v_proj", true, true, true},          {"attn_output", "self_attn.o_proj", true, true, true},
+    {"attn_q_norm", "self_attn.q_norm", false, false, true},   {"attn_k_norm", "self_attn.k_norm", false, false, true},
+    {"ffn_gate", "mlp.gate_proj", true, true, true},           {"ffn_up", "mlp.up_proj", true, true, true},
+    {"ffn_down", "mlp.down_proj", true, true, true},           {"ffn_gate_inp", "block_sparse_moe.gate", true, false, false},
+};
+// Mixtral's expert stacks: GGUF base name -> the per-expert HF name (HF's Mixtral files: w1 gate, w3 up, w2 down).
+const HfName kExpertNames[] = {
+    {"ffn_gate_exps", "w1", true, false, false}, {"ffn_up_exps", "w3", true, false, false}, {"ffn_down_exps", "w2", true, false, false}};
+
+}  // namespace
+
+Index to_hf_layout(Index ix, uint32_t flags) {
+  if (!(flags & KK_LOAD_HF_LAYOUT)) return ix;
+  if (ix.format != "gguf") fail(KK_EINVAL, "KK_LOAD_HF_LAYOUT applies to GGUF checkpoints only (this one is %s)", ix.format.c_str());
+  const GgufMeta& M = ix.gguf;
+  if (!M.arch.seen) fail(KK_EFORMAT, "KK_LOAD_HF_LAYOUT: the GGUF metadata has no general.architecture");
+  if (M.arch.err) fail(M.arch.err, "KK_LOAD_HF_LAYOUT: %s", M.arch.why.c_str());
+  const std::string& arch = M.arch.s;
+  const bool llama = arch == "llama", qwen2 = arch == "qwen2", qwen3 = arch == "qwen3";
+  if (!llama && !qwen2 && !qwen3)
+    fail(KK_EUNSUPPORTED, "KK_LOAD_HF_LAYOUT: architecture \"%s\" is not supported (llama, qwen2 and qwen3 are)", arch.c_str());
+  uint32_t n_head = 0, n_head_kv = 0;
+  if (llama) {  // the Q/K row permutation is llama.cpp's for the llama architecture only; qwen's NEOX rotary keeps the rows
+    n_head = need_key(M.head_count, (arch + ".attention.head_count").c_str());
+    n_head_kv = M.head_count_kv.seen ? need_key(M.head_count_kv, (arch + ".attention.head_count_kv").c_str()) : n_head;
+  }
+  std::vector<TensorRec> out;
+  out.reserve(ix.tensors.size());
+  std::set<std::string> names;
+  for (TensorRec& t : ix.tensors) {
+    const std::string& n = t.name;
+    std::string hf;
+    if (n == "token_embd.weight") hf = "model.embed_tokens.weight";
+    else if (n == "output_norm.weight") hf = "model.norm.weight";
+    else if (n == "output.weight") hf = "lm_head.weight";
+    else if (n == "rope_freqs.weight") hf = n;
+    else {
+      // blk.N.<base>.weight|bias
+      const size_t d0 = 4, d1 = n.find('.', d0);
+      const size_t sfx = n.rfind('.');
+      const bool layered = n.compare(0, 4, "blk.") == 0 && d1 != std::string::npos && d1 > d0 && sfx > d1 + 1 &&
+                           std::all_of(n.begin() + (long)d0, n.begin() + (long)d1, [](char ch) { return ch >= '0' && ch <= '9'; });
+      const std::string suffix = layered ? n.substr(sfx) : "";
+      if (layered && (suffix == ".weight" || suffix == ".bias")) {
+        const std::string layer = n.substr(d0, d1 - d0), base = n.substr(d1 + 1, sfx - d1 - 1);
+        const std::string prefix = "model.layers." + layer + ".";
+        auto in_arch = [&](const HfName& e) { return (llama && e.llama) || (qwen2 && e.qwen2) || (qwen3 && e.qwen3); };
+        for (auto& e : kLayerNames)
+          if (base == e.gguf && in_arch(e)) hf = prefix + e.hf + suffix;
+        bool split = false;
+        for (auto& e : kExpertNames) {
+          if (base != e.gguf || !in_arch(e) || suffix != ".weight") continue;
+          if (t.shape.size() != 3 || t.shape[0] == 0)
+            fail(KK_EFORMAT, "KK_LOAD_HF_LAYOUT: expert stack %s is not [experts, rows, cols]", n.c_str());
+          const uint64_t E = t.shape[0];
+          if (M.expert_count.seen && need_key(M.expert_count, (arch + ".expert_count").c_str()) != E)
+            fail(KK_EFORMAT, "KK_LOAD_HF_LAYOUT: expert stack %s has %llu experts, %s.expert_count says %llu", n.c_str(), (unsigned long long)E,
+                 arch.c_str(), (unsigned long long)M.expert_count.u);
+          for (uint64_t x = 0; x < E; ++x) {  // each expert is a whole number of rows, so a contiguous byte range of the stack
+            TensorRec r;
+            r.name = prefix + "block_sparse_moe.experts." + std::to_string(x) + "." + e.hf + ".weight";
+            r.dtype = t.dtype;
+            r.shape = {t.shape[1], t.shape[2]};
+            r.shard = t.shard;
+            r.nbytes = t.nbytes / E;
+            r.file_offset = t.file_offset + x * r.nbytes;
+            if (!names.insert(r.name).second) fail(KK_EFORMAT, "KK_LOAD_HF_LAYOUT: two tensors map to %s", r.name.c_str());
+            out.push_back(std::move(r));
+          }
+          split = true;
+        }
+        if (split) continue;
+        const bool q = base == "attn_q", k = base == "attn_k";
+        if (llama && (q || k) && !hf.empty()) {
+          const uint32_t heads = q ? n_head : n_head_kv;
+          const uint64_t rows = t.shape.empty() ? 0 : t.shape[0];
+          if (t.shape.empty() || t.shape.size() > 2 || rows % (2ull * heads) != 0)
+            fail(KK_EFORMAT, "KK_LOAD_HF_LAYOUT: %s has %llu rows, not a multiple of 2 * %u heads", n.c_str(), (unsigned long long)rows, heads);
+          // the rows are moved one by one, so each must be a whole number of the op's source units: a block-quantised row holds whole
+          // blocks (a 1-D block-quantised tensor, whose rows are single elements, cannot be un-permuted)
+          const DtypeInfo* di = dtype_info(t.dtype);
+          const uint64_t row_elems = t.shape.size() == 2 ? t.shape[1] : 1;
+          if (!di || di->block_bytes == 0 || row_elems % di->block_elems != 0)
+            fail(KK_EUNSUPPORTED, "KK_LOAD_HF_LAYOUT: %s (%s, shape of %zu dims) has rows that are not whole %s blocks; its rows cannot be un-permuted",
+                 n.c_str(), di ? di->name : "?", t.shape.size(), di ? di->name : "?");
+          t.rope_heads = heads;
+        }
+      }
+    }
+    if (hf.empty()) fail(KK_EUNSUPPORTED, "KK_LOAD_HF_LAYOUT: tensor %s has no Hugging Face name for architecture %s", n.c_str(), arch.c_str());
+    if (!names.insert(hf).second) fail(KK_EFORMAT, "KK_LOAD_HF_LAYOUT: two tensors map to %s", hf.c_str());
+    t.name = std::move(hf);
+    out.push_back(std::move(t));
+  }
+  ix.tensors = std::move(out);
+  ix.hf_arch = arch;
+  return ix;
+}
+
+namespace {
+
+// Pieces of a tensor whose rows llama.cpp interleaved per rotary half (TensorRec::rope_heads), for HF rows [r0, r1) of it with HF row r0 at
+// pool offset dst.  HF row h*hd + k*hd/2 + i is file row h*hd + 2i + k, so the rows of one (head, half) group are one strided run of file rows.
+// The pieces come in HF row order and tile [r0, r1) exactly: destination offsets never decrease in plan order (a part stays one pool range)
+// and every pool byte of the slice is written once.  A slice boundary may cut a group (scatter does not need heads % ranks == 0).
+void unpermuted_pieces(const TensorRec& t, const Piece& whole, uint64_t r0, uint64_t r1, uint64_t dst, std::vector<Piece>& out) {
+  const uint64_t R = t.shape[0], half = R / t.rope_heads / 2, row_bytes = t.nbytes / R;
+  const uint64_t row_units = row_bytes / whole.oi.src_unit_bytes, out_row = row_units * whole.oi.out_unit_bytes;
+  if (row_bytes * R != t.nbytes || row_units * whole.oi.src_unit_bytes != row_bytes || row_units == 0)  // to_hf_layout refuses such tensors
+    fail(KK_EUNSUPPORTED, "KK_LOAD_HF_LAYOUT: tensor %s: a row is not a whole number of source units", t.name.c_str());
+  for (uint64_t g = r0 / half; g * half < r1; ++g) {
+    const uint64_t a = std::max(r0, g * half), b = std::min(r1, (g + 1) * half);
+    const uint64_t head = g / 2, k = g % 2, i0 = a - g * half;
+    Piece pc = whole;
+    pc.file_off = t.file_offset + (head * 2 * half + 2 * i0 + k) * row_bytes;
+    pc.run_bytes = row_bytes;
+    pc.n_runs = b - a;
+    pc.stride = 2 * row_bytes;
+    pc.units = (b - a) * row_units;
+    pc.dst_off = dst + (a - r0) * out_row;
+    // the consumers store whole 16-byte vectors from a segment's first output on
+    if (pc.dst_off % 16 != 0)
+      fail(KK_EUNSUPPORTED, "KK_LOAD_HF_LAYOUT: tensor %s: HF row %llu would start at pool offset %llu, off a 16-byte boundary (%llu B per row)",
+           t.name.c_str(), (unsigned long long)a, (unsigned long long)pc.dst_off, (unsigned long long)out_row);
+    out.push_back(pc);
+  }
+}
+
+}  // namespace
+
 Plan build_plan(Index index, int mode, uint32_t flags, int n_parts, uint64_t chunk_bytes) {
   if (n_parts < 1 || n_parts > KK_MAX_DEVICES) fail(KK_EINVAL, "n_parts %d out of range", n_parts);
   if (mode != KK_MODE_SINGLE && mode != KK_MODE_BROADCAST && mode != KK_MODE_SCATTER) fail(KK_EINVAL, "unknown mode %d", mode);
@@ -474,8 +619,13 @@ Plan build_plan(Index index, int mode, uint32_t flags, int n_parts, uint64_t chu
       p.pool_offset = off;
       pc.dst_off = off;
       off = align_up(off + p.nbytes, KK_POOL_ALIGN);
+      if (t.rope_heads && !tr && p.nbytes) {  // the same slot, filled in HF row order (a dim-0 slice keeps HF rows)
+        const uint64_t r0 = p.slice_dim == 0 ? p.slice_begin : 0;
+        unpermuted_pieces(t, pc, r0, r0 + p.shape[0], p.pool_offset, pieces[(size_t)L]);
+      } else {
+        pieces[(size_t)L].push_back(pc);
+      }
       pl.push_back(std::move(p));
-      pieces[(size_t)L].push_back(pc);
     }
     P.pool_bytes[(size_t)L] = off ? off : KK_POOL_ALIGN;
   }
@@ -570,6 +720,7 @@ std::string plan_to_json(const Plan& P) {
   std::ostringstream o;
   o << "{\"mode\":" << P.mode << ",\"flags\":" << P.flags << ",\"n_parts\":" << P.n_parts << ",\"file_bytes\":" << P.file_bytes
     << ",\"format\":\"" << P.index.format << "\"";
+  if (!P.index.hf_arch.empty()) o << ",\"layout\":\"hf\",\"architecture\":\"" << json_escape(P.index.hf_arch) << "\"";
   if (P.index.layer_end) o << ",\"layers\":[" << P.index.layer_begin << "," << P.index.layer_end << "],\"n_layers\":" << P.index.n_layers;
   o << ",\"shards\":[";
   for (size_t i = 0; i < P.index.shards.size(); ++i) o << (i ? "," : "") << "\"" << json_escape(P.index.shards[i]) << "\"";

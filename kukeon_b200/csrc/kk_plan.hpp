@@ -72,6 +72,13 @@ uint32_t scatter_slice_dim(const TensorRec& t, int n_parts);
 // Throws KK_EINVAL (empty or out-of-range range) and KK_EUNSUPPORTED (no layered tensors, or two numbered stacks).
 Index select_layers(Index index, uint32_t layer_begin, uint32_t layer_end);
 
+// The Hugging Face view of a GGUF checkpoint under KK_LOAD_HF_LAYOUT (the rule is documented next to the flag in kukeon_gpuload.h); any
+// other flags return the index unchanged.  Renames every tensor, splits each expert stack into one record per expert (a byte range of the
+// stack) and marks llama's Q/K tensors (TensorRec::rope_heads) for build_plan to un-permute; the index order stays (shard, file offset).
+// Throws KK_EINVAL (not a GGUF checkpoint), KK_EFORMAT (a needed metadata key missing or ill-typed, Q/K rows not a multiple of 2 * heads)
+// and KK_EUNSUPPORTED (an architecture or a tensor outside the table).  Runs before select_layers.
+Index to_hf_layout(Index index, uint32_t flags);
+
 // JSON description of a plan (kk_plan_describe).
 std::string plan_to_json(const Plan& P);
 

@@ -26,6 +26,7 @@ CFG_ZEROCOPY, CFG_NO_PEER_ACCESS, CFG_NO_NUMA_PIN, CFG_PEER_ALL, CFG_VMM_POOLS =
 IMPORT_READONLY = 0x1
 LOAD_GPT2_CONV1D_T, LOAD_KEEP_F32, LOAD_DEFER, LOAD_SCATTER_EXCHANGE, LOAD_F8_TO_BF16 = 0x1, 0x2, 0x4, 0x8, 0x10
 LOAD_F16 = 0x80  # every float output as IEEE fp16 instead of bf16, same pool layout (kukeon_gpuload.h KK_LOAD_F16); 0x20 / 0x40 stay unused
+LOAD_HF_LAYOUT = 0x100  # GGUF in Hugging Face layout: HF names, one tensor per expert, llama's Q/K rows un-permuted (KK_LOAD_HF_LAYOUT)
 BUF_POOL, BUF_RAW, BUF_POOL_PTR, BUF_SLICE, BUF_SLICE_PTR = 0, 1, 2, 3, 4
 PROBE_WRITE, PROBE_COPY = 0, 1
 

@@ -72,7 +72,7 @@ def Load(pool: gpupool.Pool, ref: ModelRef | str, mode: int = MODE_SINGLE, fanou
     """Make the checkpoint resident in the pool(s).  Returns a refcounted Model; a second Load of the same
     checkpoint returns the same resident copy with its count bumped.  layers=(begin, end) loads only that pipeline
     stage, as a model of its own.  flags are gpupool.LOAD_*: LOAD_F16 stores every float output as fp16 instead of bf16
-    (a model apart from the bf16 load of the same file)."""
+    (a model apart from the bf16 load of the same file); LOAD_HF_LAYOUT loads a GGUF checkpoint under Hugging Face names and layout."""
     path = ref.path if isinstance(ref, ModelRef) else ref
     return pool.load(path, mode=mode, fanout=fanout, flags=flags, part_index=part_index, part_count=part_count, layers=layers)
 

@@ -30,7 +30,7 @@ from . import gpupool
 DEFAULT_TARGET = "/run/kukeon/gpupool"
 MODES = {"": gpupool.MODE_SINGLE, "single": gpupool.MODE_SINGLE, "broadcast": gpupool.MODE_BROADCAST, "scatter": gpupool.MODE_SCATTER}
 OPTION_FLAGS = {"gpt2Conv1dTranspose": gpupool.LOAD_GPT2_CONV1D_T, "keepF32": gpupool.LOAD_KEEP_F32, "f8ToBf16": gpupool.LOAD_F8_TO_BF16,
-                "f16": gpupool.LOAD_F16}
+                "f16": gpupool.LOAD_F16, "hfLayout": gpupool.LOAD_HF_LAYOUT}
 
 
 MODEL_NAME_RE = re.compile(r"^[A-Za-z0-9][A-Za-z0-9._-]*$")

@@ -74,6 +74,12 @@ int main(int argc, char** argv) {
           kk::Plan P = kk::build_plan(ix, mode, (uint32_t)(rng() % 16) & ~4u, parts, (1ull << 20) * (1 + rng() % 4));
           (void)kk::plan_to_json(P);
         } catch (const kk::Error&) {}
+        // the HF view reads the GGUF metadata keys and the tensor names and shapes the mutations reach
+        try {
+          kk::Plan P = kk::build_plan(kk::to_hf_layout(ix, KK_LOAD_HF_LAYOUT), mode, KK_LOAD_HF_LAYOUT | ((uint32_t)(rng() % 16) & ~4u), parts,
+                                      (1ull << 20) * (1 + rng() % 4));
+          (void)kk::plan_to_json(P);
+        } catch (const kk::Error&) {}
       }
       ++ok;
     } catch (const kk::Error&) {

@@ -182,6 +182,41 @@ def mixtral_gguf_tensors(hidden: int = 4096, ffn: int = 14336, layers: int = 32,
     return t
 
 
+def llama_gguf_tensors(hidden: int, ffn: int, layers: int, n_head: int, n_head_kv: int, vocab: int, head_dim: int = 0, qtype: str = "BF16",
+                       arch: str = "llama", experts: int = 0, bias: bool = False, bias_types: Sequence[str] = ("F32", "F32", "F32")):
+    """llama.cpp naming of a llama / qwen2 / qwen3 model (Mixtral with experts > 0) with explicit head counts; head_dim defaults to
+    hidden / n_head (Mistral-Nemo has another).  Norms and the router are F32, the q / k / v biases bias_types, every other weight qtype."""
+    hd = head_dim or hidden // n_head
+    t = [("token_embd.weight", qtype, [vocab, hidden])]
+    for i in range(layers):
+        p = f"blk.{i}."
+        t += [(p + "attn_norm.weight", "F32", [hidden]), (p + "attn_q.weight", qtype, [n_head * hd, hidden]),
+              (p + "attn_k.weight", qtype, [n_head_kv * hd, hidden]), (p + "attn_v.weight", qtype, [n_head_kv * hd, hidden])]
+        if bias:
+            t += [(p + "attn_q.bias", bias_types[0], [n_head * hd]), (p + "attn_k.bias", bias_types[1], [n_head_kv * hd]),
+                  (p + "attn_v.bias", bias_types[2], [n_head_kv * hd])]
+        if arch == "qwen3":
+            t += [(p + "attn_q_norm.weight", "F32", [hd]), (p + "attn_k_norm.weight", "F32", [hd])]
+        t += [(p + "attn_output.weight", qtype, [hidden, n_head * hd]), (p + "ffn_norm.weight", "F32", [hidden])]
+        if experts:
+            t += [(p + "ffn_gate_inp.weight", "F32", [experts, hidden]), (p + "ffn_gate_exps.weight", qtype, [experts, ffn, hidden]),
+                  (p + "ffn_up_exps.weight", qtype, [experts, ffn, hidden]), (p + "ffn_down_exps.weight", qtype, [experts, hidden, ffn])]
+        else:
+            t += [(p + "ffn_gate.weight", qtype, [ffn, hidden]), (p + "ffn_up.weight", qtype, [ffn, hidden]), (p + "ffn_down.weight", qtype, [hidden, ffn])]
+    t += [("output_norm.weight", "F32", [hidden]), ("output.weight", qtype, [vocab, hidden])]
+    return t
+
+
+def gguf_head_kv(arch: str, n_head: int, n_head_kv: int = 0, experts: int = 0):
+    """extra_kv entries for write_gguf: <arch>.attention.head_count(_kv) and <arch>.expert_count as UINT32."""
+    kv = [(f"{arch}.attention.head_count", 4, struct.pack("<I", n_head))]
+    if n_head_kv:
+        kv.append((f"{arch}.attention.head_count_kv", 4, struct.pack("<I", n_head_kv)))
+    if experts:
+        kv.append((f"{arch}.expert_count", 4, struct.pack("<I", experts)))
+    return kv
+
+
 def _gguf_str(s: str) -> bytes:
     b = s.encode("utf-8")
     return struct.pack("<Q", len(b)) + b
