@@ -130,8 +130,8 @@ int kk_plan_describe(kk_ctx*, const char* path, const kk_load_opts* opts, int n_
     need(path, "path");
     need(opts, "opts");
     if (chunk_bytes == 0) chunk_bytes = 64ull << 20;
-    kk::Plan P = kk::build_plan(kk::select_layers(kk::to_hf_layout(kk::index_path(path), opts->flags), opts->layer_begin, opts->layer_end), opts->mode,
-                                opts->flags & ~KK_LOAD_DEFER, n_parts, chunk_bytes);
+    kk::Plan P = kk::build_plan(kk::index_for_load(path, opts->flags, opts->layer_begin, opts->layer_end), opts->mode, opts->flags & ~KK_LOAD_DEFER,
+                                n_parts, chunk_bytes);
     std::string s = kk::plan_to_json(P);
     if (required) *required = s.size() + 1;
     if (!json) return;

@@ -547,4 +547,197 @@ Index index_path(const std::string& path_in) {
   return index_files("", {path}, false);
 }
 
+// ---------------------------------------------------------------------------------------------
+// Views of an index: the Hugging Face layout and a pipeline stage
+// ---------------------------------------------------------------------------------------------
+namespace {
+
+// Layer of a tensor: the first dotted component pair "<container>.<N>." with <container> one of layers / h / blk and N all digits.
+// stack receives the name up to and including "<container>.", which names the numbered stack the layer belongs to.
+bool layer_of(const std::string& n, uint64_t& layer, std::string& stack) {
+  size_t c = 0;  // start of the current component
+  while (c < n.size()) {
+    const size_t dot = n.find('.', c);
+    if (dot == std::string::npos) return false;
+    const std::string comp = n.substr(c, dot - c);
+    if (comp == "layers" || comp == "h" || comp == "blk") {
+      const size_t d0 = dot + 1, d1 = n.find('.', d0);
+      if (d1 != std::string::npos && d1 > d0 &&
+          std::all_of(n.begin() + (long)d0, n.begin() + (long)d1, [](char ch) { return ch >= '0' && ch <= '9'; })) {
+        layer = 0;
+        for (size_t i = d0; i < d1; ++i) layer = std::min<uint64_t>(layer * 10 + (uint64_t)(n[i] - '0'), 0xFFFFFFFFull);  // beyond any layer_end
+        stack = n.substr(0, dot + 1);
+        return true;
+      }
+    }
+    c = dot + 1;
+  }
+  return false;
+}
+
+}  // namespace
+
+Index select_layers(Index ix, uint32_t begin, uint32_t end) {
+  if (end == 0 && begin == 0) return ix;
+  if (end == 0) fail(KK_EINVAL, "layer range [%u, 0): layer_end 0 selects the whole checkpoint and takes layer_begin 0", begin);
+  if (begin >= end) fail(KK_EINVAL, "layer range [%u, %u) is empty", begin, end);
+  std::string stack;
+  uint64_t n_layers = 0;
+  bool has_head = false;
+  std::vector<uint64_t> layer(ix.tensors.size(), UINT64_MAX);  // UINT64_MAX: outer tensor
+  for (size_t i = 0; i < ix.tensors.size(); ++i) {
+    const std::string& n = ix.tensors[i].name;
+    std::string s;
+    if (layer_of(n, layer[i], s)) {
+      if (stack.empty()) stack = s;
+      else if (s != stack)
+        fail(KK_EUNSUPPORTED, "the checkpoint has two numbered layer stacks, \"%s\" and \"%s\" (tensor %s): a layer range cannot tell which to cut",
+             stack.c_str(), s.c_str(), n.c_str());
+      n_layers = std::max(n_layers, layer[i] + 1);
+    }
+    has_head = has_head || ends_with(n, "lm_head.weight") || n == "output.weight";
+  }
+  if (stack.empty()) fail(KK_EUNSUPPORTED, "layer range [%u, %u): the checkpoint has no tensor with a layer index (layers.N. / h.N. / blk.N.)", begin, end);
+  if (end > n_layers) fail(KK_EINVAL, "layer range [%u, %u) exceeds the checkpoint's %llu layers", begin, end, (unsigned long long)n_layers);
+  const bool first = begin == 0, last = end == n_layers;
+  auto any_suffix = [](const std::string& n, std::initializer_list<const char*> sufs) {
+    for (auto s : sufs)
+      if (ends_with(n, s)) return true;
+    return false;
+  };
+  std::vector<TensorRec> kept;
+  for (size_t i = 0; i < ix.tensors.size(); ++i) {
+    const std::string& n = ix.tensors[i].name;
+    bool keep;
+    if (layer[i] != UINT64_MAX) keep = layer[i] >= begin && layer[i] < end;
+    else if (any_suffix(n, {"embed_tokens.weight", "token_embd.weight", "wte.weight"})) keep = first || (last && !has_head);  // tied head
+    else if (ends_with(n, "wpe.weight")) keep = first;
+    else if (n == "output.weight" || any_suffix(n, {"lm_head.weight", "lm_head.bias", "norm.weight", "norm.bias", "ln_f.weight", "ln_f.bias"}))
+      keep = last;
+    else keep = true;  // e.g. GGUF rope_freqs.weight: every stage
+    if (keep) kept.push_back(std::move(ix.tensors[i]));
+  }
+  ix.tensors = std::move(kept);
+  ix.layer_begin = begin;
+  ix.layer_end = end;
+  ix.n_layers = n_layers;
+  return ix;
+}
+
+namespace {
+
+uint32_t need_key(const GgufKey& k, const char* key) {
+  if (!k.seen) fail(KK_EFORMAT, "KK_LOAD_HF_LAYOUT: the GGUF metadata has no %s", key);
+  if (k.err) fail(k.err, "KK_LOAD_HF_LAYOUT: %s", k.why.c_str());
+  return (uint32_t)k.u;
+}
+
+// The rename table, restated from gguf-py's tensor_mapping for llama / qwen2 / qwen3: per-layer GGUF base name -> HF name under
+// model.layers.N., and which architectures carry it.
+struct HfName { const char* gguf; const char* hf; bool llama, qwen2, qwen3; };
+const HfName kLayerNames[] = {
+    {"attn_norm", "input_layernorm", true, true, true},        {"ffn_norm", "post_attention_layernorm", true, true, true},
+    {"attn_q", "self_attn.q_proj", true, true, true},          {"attn_k", "self_attn.k_proj", true, true, true},
+    {"attn_v", "self_attn.v_proj", true, true, true},          {"attn_output", "self_attn.o_proj", true, true, true},
+    {"attn_q_norm", "self_attn.q_norm", false, false, true},   {"attn_k_norm", "self_attn.k_norm", false, false, true},
+    {"ffn_gate", "mlp.gate_proj", true, true, true},           {"ffn_up", "mlp.up_proj", true, true, true},
+    {"ffn_down", "mlp.down_proj", true, true, true},           {"ffn_gate_inp", "block_sparse_moe.gate", true, false, false},
+};
+// Mixtral's expert stacks: GGUF base name -> the per-expert HF name (HF's Mixtral files: w1 gate, w3 up, w2 down).
+const HfName kExpertNames[] = {
+    {"ffn_gate_exps", "w1", true, false, false}, {"ffn_up_exps", "w3", true, false, false}, {"ffn_down_exps", "w2", true, false, false}};
+
+}  // namespace
+
+Index to_hf_layout(Index ix, uint32_t flags) {
+  if (!(flags & KK_LOAD_HF_LAYOUT)) return ix;
+  if (ix.format != "gguf") fail(KK_EINVAL, "KK_LOAD_HF_LAYOUT applies to GGUF checkpoints only (this one is %s)", ix.format.c_str());
+  const GgufMeta& M = ix.gguf;
+  if (!M.arch.seen) fail(KK_EFORMAT, "KK_LOAD_HF_LAYOUT: the GGUF metadata has no general.architecture");
+  if (M.arch.err) fail(M.arch.err, "KK_LOAD_HF_LAYOUT: %s", M.arch.why.c_str());
+  const std::string& arch = M.arch.s;
+  const bool llama = arch == "llama", qwen2 = arch == "qwen2", qwen3 = arch == "qwen3";
+  if (!llama && !qwen2 && !qwen3)
+    fail(KK_EUNSUPPORTED, "KK_LOAD_HF_LAYOUT: architecture \"%s\" is not supported (llama, qwen2 and qwen3 are)", arch.c_str());
+  uint32_t n_head = 0, n_head_kv = 0;
+  if (llama) {  // the Q/K row permutation is llama.cpp's for the llama architecture only; qwen's NEOX rotary keeps the rows
+    n_head = need_key(M.head_count, (arch + ".attention.head_count").c_str());
+    n_head_kv = M.head_count_kv.seen ? need_key(M.head_count_kv, (arch + ".attention.head_count_kv").c_str()) : n_head;
+  }
+  std::vector<TensorRec> out;
+  out.reserve(ix.tensors.size());
+  std::set<std::string> names;
+  for (TensorRec& t : ix.tensors) {
+    const std::string& n = t.name;
+    std::string hf;
+    if (n == "token_embd.weight") hf = "model.embed_tokens.weight";
+    else if (n == "output_norm.weight") hf = "model.norm.weight";
+    else if (n == "output.weight") hf = "lm_head.weight";
+    else if (n == "rope_freqs.weight") hf = n;
+    else {
+      // blk.N.<base>.weight|bias
+      const size_t d0 = 4, d1 = n.find('.', d0);
+      const size_t sfx = n.rfind('.');
+      const bool layered = n.compare(0, 4, "blk.") == 0 && d1 != std::string::npos && d1 > d0 && sfx > d1 + 1 &&
+                           std::all_of(n.begin() + (long)d0, n.begin() + (long)d1, [](char ch) { return ch >= '0' && ch <= '9'; });
+      const std::string suffix = layered ? n.substr(sfx) : "";
+      if (layered && (suffix == ".weight" || suffix == ".bias")) {
+        const std::string layer = n.substr(d0, d1 - d0), base = n.substr(d1 + 1, sfx - d1 - 1);
+        const std::string prefix = "model.layers." + layer + ".";
+        auto in_arch = [&](const HfName& e) { return (llama && e.llama) || (qwen2 && e.qwen2) || (qwen3 && e.qwen3); };
+        for (auto& e : kLayerNames)
+          if (base == e.gguf && in_arch(e)) hf = prefix + e.hf + suffix;
+        bool split = false;
+        for (auto& e : kExpertNames) {
+          if (base != e.gguf || !in_arch(e) || suffix != ".weight") continue;
+          if (t.shape.size() != 3 || t.shape[0] == 0)
+            fail(KK_EFORMAT, "KK_LOAD_HF_LAYOUT: expert stack %s is not [experts, rows, cols]", n.c_str());
+          const uint64_t E = t.shape[0];
+          if (M.expert_count.seen && need_key(M.expert_count, (arch + ".expert_count").c_str()) != E)
+            fail(KK_EFORMAT, "KK_LOAD_HF_LAYOUT: expert stack %s has %llu experts, %s.expert_count says %llu", n.c_str(), (unsigned long long)E,
+                 arch.c_str(), (unsigned long long)M.expert_count.u);
+          for (uint64_t x = 0; x < E; ++x) {  // each expert is a whole number of rows, so a contiguous byte range of the stack
+            TensorRec r;
+            r.name = prefix + "block_sparse_moe.experts." + std::to_string(x) + "." + e.hf + ".weight";
+            r.dtype = t.dtype;
+            r.shape = {t.shape[1], t.shape[2]};
+            r.shard = t.shard;
+            r.nbytes = t.nbytes / E;
+            r.file_offset = t.file_offset + x * r.nbytes;
+            if (!names.insert(r.name).second) fail(KK_EFORMAT, "KK_LOAD_HF_LAYOUT: two tensors map to %s", r.name.c_str());
+            out.push_back(std::move(r));
+          }
+          split = true;
+        }
+        if (split) continue;
+        const bool q = base == "attn_q", k = base == "attn_k";
+        if (llama && (q || k) && !hf.empty()) {
+          const uint32_t heads = q ? n_head : n_head_kv;
+          const uint64_t rows = t.shape.empty() ? 0 : t.shape[0];
+          if (t.shape.empty() || t.shape.size() > 2 || rows % (2ull * heads) != 0)
+            fail(KK_EFORMAT, "KK_LOAD_HF_LAYOUT: %s has %llu rows, not a multiple of 2 * %u heads", n.c_str(), (unsigned long long)rows, heads);
+          // the rows are moved one by one, so each must be a whole number of the op's source units: a block-quantised row holds whole
+          // blocks (a 1-D block-quantised tensor, whose rows are single elements, cannot be un-permuted)
+          const DtypeInfo* di = dtype_info(t.dtype);
+          const uint64_t row_elems = t.shape.size() == 2 ? t.shape[1] : 1;
+          if (!di || di->block_bytes == 0 || row_elems % di->block_elems != 0)
+            fail(KK_EUNSUPPORTED, "KK_LOAD_HF_LAYOUT: %s (%s, shape of %zu dims) has rows that are not whole %s blocks; its rows cannot be un-permuted",
+                 n.c_str(), di ? di->name : "?", t.shape.size(), di ? di->name : "?");
+          t.rope_heads = heads;
+        }
+      }
+    }
+    if (hf.empty()) fail(KK_EUNSUPPORTED, "KK_LOAD_HF_LAYOUT: tensor %s has no Hugging Face name for architecture %s", n.c_str(), arch.c_str());
+    if (!names.insert(hf).second) fail(KK_EFORMAT, "KK_LOAD_HF_LAYOUT: two tensors map to %s", hf.c_str());
+    t.name = std::move(hf);
+    out.push_back(std::move(t));
+  }
+  ix.tensors = std::move(out);
+  ix.hf_arch = arch;
+  return ix;
+}
+
+Index index_for_load(const std::string& path, uint32_t flags, uint32_t layer_begin, uint32_t layer_end) {
+  return select_layers(to_hf_layout(index_path(path), flags), layer_begin, layer_end);
+}
 }  // namespace kk

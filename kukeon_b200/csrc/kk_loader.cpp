@@ -787,7 +787,7 @@ kk_model* model_load(kk_ctx* c, const std::string& path, const kk_load_opts& opt
   const LoadShape& S = m->shape;
   try {
     double t0 = now_s();
-    Index ix = select_layers(to_hf_layout(index_path(path), opts.flags), opts.layer_begin, opts.layer_end);
+    Index ix = index_for_load(path, opts.flags, opts.layer_begin, opts.layer_end);
     m->t_index = now_s() - t0;
     t0 = now_s();
     m->plan = build_plan(std::move(ix), opts.mode, opts.flags & ~KK_LOAD_DEFER, S.n_parts, c->slot_bytes);

@@ -63,27 +63,8 @@ struct Plan {
 // chunk_bytes: staging slot size (upper bound on Chunk::buf_bytes).
 Plan build_plan(Index index, int mode, uint32_t flags, int n_parts, uint64_t chunk_bytes);
 
-// Which dimension a tensor is sliced along in SCATTER mode (kNoSlice = replicate). [PROPOSED] rule of
-// SURVEY.md §8(a3.S5): column-parallel weights along dim 0, row-parallel weights along dim 1.
-uint32_t scatter_slice_dim(const TensorRec& t, int n_parts);
-
-// Pipeline stage [layer_begin, layer_end) of a checkpoint (the rule is documented next to kk_load_opts in kukeon_gpuload.h).  Keeps the
-// shard list, every kept record's shard index and the index order; layer_end == 0 with layer_begin == 0 returns the index unchanged.
-// Throws KK_EINVAL (empty or out-of-range range) and KK_EUNSUPPORTED (no layered tensors, or two numbered stacks).
-Index select_layers(Index index, uint32_t layer_begin, uint32_t layer_end);
-
-// The Hugging Face view of a GGUF checkpoint under KK_LOAD_HF_LAYOUT (the rule is documented next to the flag in kukeon_gpuload.h); any
-// other flags return the index unchanged.  Renames every tensor, splits each expert stack into one record per expert (a byte range of the
-// stack) and marks llama's Q/K tensors (TensorRec::rope_heads) for build_plan to un-permute; the index order stays (shard, file offset).
-// Throws KK_EINVAL (not a GGUF checkpoint), KK_EFORMAT (a needed metadata key missing or ill-typed, Q/K rows not a multiple of 2 * heads)
-// and KK_EUNSUPPORTED (an architecture or a tensor outside the table).  Runs before select_layers.
-Index to_hf_layout(Index index, uint32_t flags);
-
 // JSON description of a plan (kk_plan_describe).
 std::string plan_to_json(const Plan& P);
-
-// True when KK_LOAD_GPT2_CONV1D_T applies to this tensor.
-bool is_gpt2_conv1d(const TensorRec& t);
 
 // How a load moves its bytes between the devices.
 enum class LoadOrder {
