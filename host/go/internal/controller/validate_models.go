@@ -87,6 +87,23 @@ func validateModels(in []intmodel.ModelMount) ([]intmodel.ModelMount, error) {
 			return nil, fmt.Errorf("failed to stat model[%d] source %q: %w", i, src, statErr)
 		}
 
+		// adapter: absent, or a PEFT LoRA adapter on the host merged into the pool on load (kk_load_adapter), validated like source
+		adapter := strings.TrimSpace(m.Adapter)
+		if m.Adapter != "" {
+			if !filepath.IsAbs(adapter) {
+				if strings.Contains(adapter, "://") || (strings.ContainsRune(adapter, os.PathSeparator) && !strings.HasPrefix(adapter, ".")) {
+					return nil, fmt.Errorf("%w (model[%d] adapter %q)", errdefs.ErrModelAdapterRegistryNotSupported, i, adapter)
+				}
+				return nil, fmt.Errorf("%w (model[%d] adapter %q)", errdefs.ErrModelAdapterNotAbsolute, i, adapter)
+			}
+			if _, statErr := os.Stat(adapter); statErr != nil {
+				if os.IsNotExist(statErr) {
+					return nil, fmt.Errorf("%w (model[%d] adapter %q)", errdefs.ErrModelAdapterNotFound, i, adapter)
+				}
+				return nil, fmt.Errorf("failed to stat model[%d] adapter %q: %w", i, adapter, statErr)
+			}
+		}
+
 		target := strings.TrimSpace(m.Target)
 		if target == "" {
 			target = defaultModelTarget
@@ -122,7 +139,7 @@ func validateModels(in []intmodel.ModelMount) ([]intmodel.ModelMount, error) {
 		}
 
 		out[i] = intmodel.ModelMount{Name: name, Source: src, Target: target, Mode: mode, Devices: append([]int(nil), m.Devices...), Options: m.Options,
-			Layers: append([]int(nil), m.Layers...)}
+			Layers: append([]int(nil), m.Layers...), Adapter: adapter}
 	}
 	return out, nil
 }

@@ -30,4 +30,7 @@ var (
 	ErrModelLayersInvalid        = errors.New("model layers must be [begin, end): two non-negative integers with begin < end")
 	ErrModelOptionUnknown        = errors.New("model option is not recognized")
 	ErrModelRegistryNotSupported = errors.New("registry references are not supported; use an absolute host path as source")
+	ErrModelAdapterNotAbsolute   = errors.New("model adapter must be an absolute host path")
+	ErrModelAdapterNotFound      = errors.New("model adapter does not exist on the host")
+	ErrModelAdapterRegistryNotSupported = errors.New("adapter registry references are not supported; use an absolute host path as adapter")
 )

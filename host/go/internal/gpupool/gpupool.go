@@ -174,8 +174,9 @@ func Plan(path string, mode Mode, flags uint32, gpus int, layers Layers) ([]byte
 }
 
 // Load makes the checkpoint resident (or returns the already-resident copy with its refcount bumped): N concurrent StartCell
-// calls for the same model share one load.  A pipeline stage (layers not zero) is a model of its own.
-func (p *Pool) Load(path string, mode Mode, flags uint32, layers Layers) (*Model, error) {
+// calls for the same model share one load.  A pipeline stage (layers not zero) is a model of its own.  adapter, when not empty, is a
+// PEFT LoRA adapter merged into the pool(s) after the load (kk_load_adapter); base + adapter is a model of its own.
+func (p *Pool) Load(path string, mode Mode, flags uint32, layers Layers, adapter string) (*Model, error) {
 	cs := C.CString(path)
 	defer C.free(unsafe.Pointer(cs))
 	var o C.kk_load_opts
@@ -185,10 +186,40 @@ func (p *Pool) Load(path string, mode Mode, flags uint32, layers Layers) (*Model
 	o.layer_begin = C.uint32_t(layers.Begin)
 	o.layer_end = C.uint32_t(layers.End)
 	m := &Model{}
-	if err := call(func() C.int { return C.kk_load_ex(p.h, cs, &o, &m.h) }); err != nil {
+	if adapter == "" {
+		if err := call(func() C.int { return C.kk_load_ex(p.h, cs, &o, &m.h) }); err != nil {
+			return nil, err
+		}
+		return m, nil
+	}
+	ca := C.CString(adapter)
+	defer C.free(unsafe.Pointer(ca))
+	if err := call(func() C.int { return C.kk_load_adapter(p.h, cs, &o, ca, &m.h) }); err != nil {
 		return nil, err
 	}
 	return m, nil
+}
+
+// AdapterDescribe validates a LoRA adapter against the checkpoint as Load would see it and returns the merge it would do as JSON
+// (kk_adapter_describe; CPU only).
+func AdapterDescribe(path string, mode Mode, flags uint32, layers Layers, adapter string) ([]byte, error) {
+	cs, ca := C.CString(path), C.CString(adapter)
+	defer C.free(unsafe.Pointer(cs))
+	defer C.free(unsafe.Pointer(ca))
+	var o C.kk_load_opts
+	o.mode = C.int32_t(mode)
+	o.flags = C.uint32_t(flags)
+	o.layer_begin = C.uint32_t(layers.Begin)
+	o.layer_end = C.uint32_t(layers.End)
+	var need C.size_t
+	if err := call(func() C.int { return C.kk_adapter_describe(nil, cs, &o, ca, nil, 0, &need) }); err != nil {
+		return nil, err
+	}
+	buf := make([]byte, need)
+	if err := call(func() C.int { return C.kk_adapter_describe(nil, cs, &o, ca, (*C.char)(unsafe.Pointer(&buf[0])), need, nil) }); err != nil {
+		return nil, err
+	}
+	return buf[:need-1], nil
 }
 
 // ExportFD returns a new file descriptor for the VMM pool of `device` and its mapped size (KK_CFG_VMM_POOLS contexts only).  The caller sends it to

@@ -161,7 +161,10 @@ class Pool {
     if (h_) { errdefs::check(kk_close(h_)); h_ = nullptr; }
   }
   // layers: the pipeline stage [begin, end) to load; {0, 0} is the whole checkpoint.  A stage is a model of its own.
-  Model Load(const std::string& path, int mode = KK_MODE_SINGLE, int fanout = KK_FANOUT_P2P, uint32_t flags = 0, Layers layers = {}) {
+  // adapter: a PEFT LoRA adapter merged into the pool(s) after the load (kk_load_adapter); empty: the checkpoint alone.  Base + adapter is a
+  // model of its own.
+  Model Load(const std::string& path, int mode = KK_MODE_SINGLE, int fanout = KK_FANOUT_P2P, uint32_t flags = 0, Layers layers = {},
+             const std::string& adapter = std::string()) {
     kk_load_opts o{};
     o.mode = mode;
     o.fanout = fanout;
@@ -169,7 +172,8 @@ class Pool {
     o.layer_begin = layers.begin;
     o.layer_end = layers.end;
     kk_model* m = nullptr;
-    errdefs::check(kk_load_ex(h_, path.c_str(), &o, &m));
+    if (adapter.empty()) errdefs::check(kk_load_ex(h_, path.c_str(), &o, &m));
+    else errdefs::check(kk_load_adapter(h_, path.c_str(), &o, adapter.c_str(), &m));
     return Model(m);
   }
   kk_ctx* handle() const { return h_; }
@@ -211,8 +215,8 @@ inline TensorIndex Pull(const std::string& path) {
 }
 
 inline gpupool::Model Load(gpupool::Pool& pool, const std::string& path, int mode = KK_MODE_SINGLE, uint32_t flags = 0,
-                           gpupool::Layers layers = {}) {
-  return pool.Load(path, mode, KK_FANOUT_P2P, flags, layers);
+                           gpupool::Layers layers = {}, const std::string& adapter = std::string()) {
+  return pool.Load(path, mode, KK_FANOUT_P2P, flags, layers, adapter);
 }
 
 struct OCIMount { std::string destination, type, source; std::vector<std::string> options; };

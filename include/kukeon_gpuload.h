@@ -272,6 +272,43 @@ int kk_plan_describe(kk_ctx* ctx, const char* path, const kk_load_opts* opts, in
 /* ---- Load ------------------------------------------------------------------------------------ */
 int kk_load(kk_ctx* ctx, const char* path, int mode, int fanout, kk_model** out);
 int kk_load_ex(kk_ctx* ctx, const char* path, const kk_load_opts* opts, kk_model** out);
+/* LoRA adapters.  kk_load_adapter loads `path` with `opts` exactly as kk_load_ex would, then merges the PEFT LoRA adapter at
+ * `adapter_path` into the pool(s) on the GPU.  kk_adapter_describe (CPU only, ctx may be NULL) validates the adapter against the checkpoint
+ * as that load would see it and describes the merge as JSON: per target its pool name, dtype, shape, r, scaling and the adapter tensors
+ * used, plus the targets skipped by the stage.  KK_ERANGE / *required as kk_plan_describe.
+ *   input     adapter_path is a directory holding adapter_config.json and adapter_model.safetensors, or that safetensors file with the
+ *             config beside it (PEFT's save_pretrained form).
+ *   names     base_model.model.<M>.lora_A.weight [r, C] and base_model.model.<M>.lora_B.weight [R, r] target pool tensor <M>.weight [R, C],
+ *             matched against the names the load plans over (HF names under KK_LOAD_HF_LAYOUT).  A target that exists in the checkpoint
+ *             but lies outside the load's layer stage is skipped; one that does not exist is KK_ENOENT.  Nothing is dropped silently.
+ *   scaling   s = (float)(lora_alpha / r), or (float)(lora_alpha / sqrt(r)) under use_rslora, computed in double and rounded once; r is
+ *             each pair's own (A's rows), so rank_pattern needs nothing.
+ *   merge     for element (i, j) of the full tensor (a SCATTER slice's slice_begin offsets i for dim 0 or j for dim 1), w the pool element
+ *             after the ordinary load widened to fp32, A and B widened exactly from their file dtype:
+ *               acc = 0.0f; for k = 0 .. r-1: acc = fmaf(B[i][k], A[k][j], acc)   (this order, no split-K; CUDA-core FFMA)
+ *               out = fmaf(s, acc, w) rounded to nearest even into the pool dtype (bf16 / f16 overflow -> inf, f32 as is); any NaN -> 0x7FFF
+ *                     (0x7FFFFFFF in an F32 pool); subnormals are kept
+ *             Bytes outside the targets are untouched, and the pool layout (placements, offsets, sizes, dtypes) is that of the same load
+ *             without the adapter.  The pool dtype follows the load: bf16, KK_LOAD_F16, KK_LOAD_KEEP_F32 and GGUF block types dequantised first.
+ *   when      at the end of kk_load_adapter (one process: after the fan-out or RAW stage 2 on every pool) and, for a KK_LOAD_DEFER model, at the
+ *             end of every kk_load_part (a repeated kk_load_part rewrites the base bytes and merges again: the result is identical).
+ *   memory    A and B are uploaded as fp32 once per device that merges, in one buffer freed before the call returns; kk_stats shows its bytes.
+ *   identity  the canonical adapter path is part of the model's identity: base + opts + adapter again is the same model (refcount + 1), the
+ *             base alone and base + adapter are two models.  The manifest and kk_stats gain an "adapter" object.
+ *   refusals  all raised before any device is touched.
+ *             KK_EUNSUPPORTED: a non-empty alpha_pattern; use_dora / lora_magnitude_vector; fan_in_fan_out; lora_embedding_A/B;
+ *                              modules_to_save tensors; bias tensors or bias other than "none"; adapter_model.bin; adapter dtypes other than
+ *                              F32 / BF16 / F16; r outside 1..256; a target that is not 2-D or whose pool dtype is not bf16, f16 or F32 (FP8 kept
+ *                              verbatim, integers, transposed GPT-2 weights); KK_FANOUT_NVLS; a part_count > 1 load whose pool receives peers'
+ *                              stores (BROADCAST in any fan-out, SCATTER with KK_LOAD_SCATTER_EXCHANGE).  Multi-part SCATTER without the
+ *                              exchange merges: a rank's pool is written by that rank only.
+ *             KK_EFORMAT:      an unpaired lora_A / lora_B, mismatched shapes, a key that is not a LoRA key, a malformed config or a missing
+ *                              or ill-typed config key (lora_alpha a finite number; use_rslora, use_dora, fan_in_fan_out booleans; bias a string).
+ *             KK_ENOENT:       no adapter at adapter_path, no adapter_config.json, a target the checkpoint does not have.
+ * kk_adapter_describe plans like kk_plan_describe with n_parts = part_count (1 when part_count <= 1). */
+int kk_load_adapter(kk_ctx* ctx, const char* path, const kk_load_opts* opts, const char* adapter_path, kk_model** out);
+int kk_adapter_describe(kk_ctx* ctx, const char* path, const kk_load_opts* opts, const char* adapter_path, char* json, size_t cap,
+                        size_t* required);
 /* Deferred / multi-process loading: after kk_load_ex(...KK_LOAD_DEFER...) and any kk_peer_attach calls,
  * move the data.  May be called again to re-load (pools are overwritten with identical bytes). */
 int kk_load_part(kk_model* m);

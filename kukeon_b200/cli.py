@@ -1,7 +1,7 @@
 """`kuke model …` — Python model of the CLI verbs row f3 of SURVEY.md §8(f) proposes, patterned on `kuke image` (cmd/kuke/image/*.go):
 
     python -m kukeon_b200.cli model pull <path> [-o table|yaml|json]          index a local checkpoint ("pull" is local-path only)
-    python -m kukeon_b200.cli model plan <path> [--mode M] [--gpus N] [--layers B:E] [-o …]
+    python -m kukeon_b200.cli model plan <path> [--mode M] [--gpus N] [--layers B:E] [--adapter DIR] [-o …]
                                                                               dry-run: pool layout and bytes per GPU, no device touched;
                                                                               --layers: only the pipeline stage of layers [B, E)
     python -m kukeon_b200.cli model validate <cell.yaml>                      check the `models:` entries of a Cell manifest
@@ -93,14 +93,26 @@ def cmd_plan(args, out) -> int:
                "tensors": len(plan["layouts"][0]["tensors"])}
     if args.layers:
         summary["layers"], summary["nLayers"] = plan["layers"], plan["n_layers"]
+    adapter = None
+    if args.adapter:
+        # one process over n GPUs: a scatter pool is planned as n parts, a broadcast pool like a single one
+        adapter = gpupool.adapter_describe(args.path, args.adapter, mode=MODES[args.mode], flags=flags, part_count=n if args.mode == "scatter" else 0,
+                                           layers=args.layers)
+        summary["adapter"] = {"path": adapter["adapter"], "targets": [{"name": t["name"], "shape": t["shape"], "r": t["r"], "scaling": t["scaling"]}
+                                                                       for t in adapter["targets"]], "skipped": adapter["skipped"]}
     fmt = parse_output(args.output)
     if fmt != "table":
-        emit(summary if not args.full else plan, fmt, out)
+        emit(summary if not args.full else (plan if adapter is None else dict(plan, adapter=adapter)), fmt, out)
         return 0
     rows = [[str(g), format_size(summary["ingestBytesPerGpu"][g]), format_size(summary["poolBytesPerGpu"][g])] for g in range(n)]
     print_table(["GPU", "INGESTS", "POOL"], rows, out)
     stage = f", layers {plan['layers'][0]}-{plan['layers'][1] - 1} of {plan['n_layers']}" if args.layers else ""
     out.write(f"{summary['tensors']} tensors, {format_size(plan['file_bytes'])} in the files, mode {args.mode}{stage}\n")
+    if adapter is not None:
+        print_table(["TARGET", "SHAPE", "R", "SCALING"], [[t["name"], "x".join(map(str, t["shape"])), str(t["r"]), f"{t['scaling']:.9g}"]
+                                                         for t in adapter["targets"]], out)
+        skipped = f", {len(adapter['skipped'])} outside the stage" if adapter["skipped"] else ""
+        out.write(f"adapter {adapter['adapter']}: {len(adapter['targets'])} tensors merged{skipped}\n")
     return 0
 
 
@@ -142,6 +154,7 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--gpus", type=int, default=1)
     p.add_argument("--option", action="append", choices=sorted(schema.OPTION_FLAGS))
     p.add_argument("--layers", type=parse_layers, metavar="B:E", help="pipeline stage: plan only layers [B, E) (half-open)")
+    p.add_argument("--adapter", metavar="DIR", help="PEFT LoRA adapter (directory or adapter_model.safetensors): list the tensors its merge targets")
     p.add_argument("--full", action="store_true", help="yaml/json: the whole plan (chunks, reads, segments) instead of the summary")
     p.add_argument("-o", "--output", default="")
     p.set_defaults(fn=cmd_plan)

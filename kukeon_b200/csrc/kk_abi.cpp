@@ -140,6 +140,25 @@ int kk_plan_describe(kk_ctx*, const char* path, const kk_load_opts* opts, int n_
   });
 }
 
+int kk_adapter_describe(kk_ctx*, const char* path, const kk_load_opts* opts, const char* adapter_path, char* json, size_t cap, size_t* required) {
+  return guard([&] {
+    need(path, "path");
+    need(opts, "opts");
+    need(adapter_path, "adapter_path");
+    kk::check_adapter_opts(*opts);
+    const int n_parts = opts->part_count > 1 ? opts->part_count : 1;
+    if (n_parts > KK_MAX_DEVICES) kk::fail(KK_EINVAL, "part_count %d out of range", opts->part_count);
+    const int mode = n_parts > 1 ? opts->mode : (opts->mode == KK_MODE_SCATTER ? KK_MODE_SCATTER : KK_MODE_SINGLE);
+    kk::Plan P = kk::build_plan(kk::index_for_load(path, opts->flags, opts->layer_begin, opts->layer_end), mode, opts->flags & ~KK_LOAD_DEFER, n_parts,
+                                64ull << 20);
+    std::string s = kk::adapter_to_json(kk::match_adapter(adapter_path, path, opts->flags, P), P);
+    if (required) *required = s.size() + 1;
+    if (!json) return;
+    if (s.size() + 1 > cap) kk::fail(KK_ERANGE, "adapter description needs %zu bytes", s.size() + 1);
+    memcpy(json, s.c_str(), s.size() + 1);
+  });
+}
+
 int kk_load(kk_ctx* ctx, const char* path, int mode, int fanout, kk_model** out) {
   kk_load_opts o{};
   o.mode = mode;
@@ -155,6 +174,19 @@ int kk_load_ex(kk_ctx* ctx, const char* path, const kk_load_opts* opts, kk_model
     need(out, "out");
     *out = nullptr;
     *out = kk::model_load(ctx, path, *opts);
+  });
+}
+
+int kk_load_adapter(kk_ctx* ctx, const char* path, const kk_load_opts* opts, const char* adapter_path, kk_model** out) {
+  return guard([&] {
+    need(ctx, "ctx");
+    need(path, "path");
+    need(opts, "opts");
+    need(adapter_path, "adapter_path");
+    need(out, "out");
+    *out = nullptr;
+    if (!*adapter_path) kk::fail(KK_EINVAL, "adapter_path is empty");
+    *out = kk::model_load(ctx, path, *opts, adapter_path);
   });
 }
 

@@ -20,6 +20,7 @@
 #include <thread>
 
 #include "kk_json.hpp"
+#include "kk_lora.cuh"
 #include "kk_read.hpp"
 
 namespace kk {
@@ -534,6 +535,71 @@ void raw_fanout_launch(kk_model* m, int li, std::vector<ConvertLaunch>& out) {
   out.push_back(L);
 }
 
+// kk_load_adapter: merge the adapter into every local pool, whose bytes are all written (the load's streams have been synchronised).  One launch
+// per device over a table of that pool's targets, all enqueued before any device is waited for.  A and B (fp32) and the table live in one
+// buffer per device, freed before this returns.
+void merge_adapter(kk_model* m) {
+  const Adapter& A = *m->adapter;
+  std::vector<uint64_t> a_off, b_off;
+  const std::vector<float> host = read_adapter_f32(A, a_off, b_off);
+  const size_t nl = m->pools.size();
+  std::vector<DevBuf> bufs(nl);
+  std::vector<EventSet> evs;
+  evs.reserve(nl);
+  uint64_t most = 0;
+  for (size_t li = 0; li < nl; ++li) {
+    Device& dev = m->ctx->devs[li];
+    const std::vector<Placement>& pl = m->plan.placement_of_part(m->shape.local_parts[li]);
+    std::vector<KKLoraTarget> T;
+    uint64_t tiles = 0;
+    for (size_t i = 0; i < A.pairs.size(); ++i) {
+      const LoraPair& p = A.pairs[i];
+      const Placement& q = pl[p.tensor];
+      KKLoraTarget t{};
+      t.w_off = q.pool_offset;
+      t.a_off = a_off[i];
+      t.b_off = b_off[i];
+      t.rows = (uint32_t)q.shape[0];
+      t.cols = (uint32_t)q.shape[1];
+      t.row0 = q.slice_dim == 0 ? (uint32_t)q.slice_begin : 0;
+      t.col0 = q.slice_dim == 1 ? (uint32_t)q.slice_begin : 0;
+      t.a_ld = (uint32_t)p.a.shape[1];
+      t.r = p.r;
+      t.s = p.s;
+      t.out = lora_out_of(q.dtype);
+      t.tile_begin = (uint32_t)tiles;
+      t.tiles_c = (t.cols + KK_LORA_TILE_C - 1) / KK_LORA_TILE_C;
+      const uint32_t n = kk_lora_tiles(t.rows, t.cols);
+      if (n == 0) continue;
+      tiles += n;
+      if (tiles >= (1ull << 31)) fail(KK_EUNSUPPORTED, "adapter: more than 2^31 merge tiles on one device");
+      T.push_back(t);
+    }
+    const uint64_t tb = align_up(T.size() * sizeof(KKLoraTarget), 256), bytes = tb + host.size() * sizeof(float);
+    KK_CUDA(cudaSetDevice(dev.ordinal));
+    bufs[li] = DevBuf(dev.ordinal, bytes, "the adapter");
+    if (!T.empty()) KK_CUDA(cudaMemcpy(bufs[li].get(), T.data(), T.size() * sizeof(KKLoraTarget), cudaMemcpyHostToDevice));
+    KK_CUDA(cudaMemcpy(bufs[li].get() + tb, host.data(), host.size() * sizeof(float), cudaMemcpyHostToDevice));
+    evs.emplace_back(2);
+    evs[li].create_all();
+    KK_CUDA(cudaEventRecord(evs[li][0], dev.stream));
+    KK_CUDA(launch_lora_merge(bufs[li].get<KKLoraTarget>(), (uint32_t)T.size(), (uint32_t)tiles, (const float*)(bufs[li].get() + tb),
+                              m->pools[li].ptr, dev.stream));
+    KK_CUDA(cudaEventRecord(evs[li][1], dev.stream));
+    most = std::max(most, bytes);
+  }
+  float worst = 0.f;
+  for (size_t li = 0; li < nl; ++li) {
+    KK_CUDA(cudaSetDevice(m->ctx->devs[li].ordinal));
+    KK_CUDA(cudaStreamSynchronize(m->ctx->devs[li].stream));
+    float ms = 0.f;
+    KK_CUDA(cudaEventElapsedTime(&ms, evs[li][0], evs[li][1]));
+    worst = std::max(worst, ms);
+  }
+  m->t_merge = worst / 1e3;
+  m->adapter_bytes = most;
+}
+
 // Close the peer buffers this process opened over CUDA IPC and forget every attached one.
 void close_peers(kk_model* m) {
   for (auto& kind : m->peer)
@@ -745,15 +811,17 @@ static void do_load(kk_model* m) {
   const double tc = now_s();
   fds.cleanup();  // part of the load: unmapping a checkpoint-sized mapping is not free
   m->t_files_close = now_s() - tc;
+  if (m->adapter) merge_adapter(m);  // every pool is complete: no load shape that merges has a second stage or a peer's stores still to come
   m->t_load = now_s() - t0;
   m->n_loads++;
   std::lock_guard<std::mutex> g(m->ctx->mu);
   if (!S.two_stage) m->loaded = true;  // a two-stage model is loaded once kk_convert_local has run
 }
 
-kk_model* model_load(kk_ctx* c, const std::string& path, const kk_load_opts& opts_in) {
+kk_model* model_load(kk_ctx* c, const std::string& path, const kk_load_opts& opts_in, const std::string& adapter_path) {
   kk_load_opts opts = opts_in;
   if (opts.part_count <= 1) { opts.part_count = 1; opts.part_index = 0; }
+  if (!adapter_path.empty()) check_adapter_opts(opts);
   LoadShape shape = resolve_load_shape(opts, c->cfg.n_devices, c->peer_ok);
   if (shape.order == LoadOrder::kNvls) {
     std::vector<int> ords(c->cfg.devices, c->cfg.devices + c->cfg.n_devices);
@@ -764,6 +832,7 @@ kk_model* model_load(kk_ctx* c, const std::string& path, const kk_load_opts& opt
   std::ostringstream ks;
   ks << canon(path) << "|m" << opts.mode << "|f" << opts.fanout << "|x" << (opts.flags & ~KK_LOAD_DEFER) << "|p" << opts.part_index << "/" << opts.part_count
      << "|l" << opts.layer_begin << ":" << opts.layer_end;
+  if (!adapter_path.empty()) ks << "|a" << canon(adapter_path);
   const std::string key = ks.str();
 
   kk_model* m = nullptr;
@@ -791,6 +860,7 @@ kk_model* model_load(kk_ctx* c, const std::string& path, const kk_load_opts& opt
     m->t_index = now_s() - t0;
     t0 = now_s();
     m->plan = build_plan(std::move(ix), opts.mode, opts.flags & ~KK_LOAD_DEFER, S.n_parts, c->slot_bytes);
+    if (!adapter_path.empty()) m->adapter.reset(new Adapter(match_adapter(adapter_path, path, opts.flags, m->plan)));
     m->t_plan = now_s() - t0;
     t0 = now_s();
     // concatenated segment table of all parts
@@ -1052,6 +1122,7 @@ static std::string build_manifest(kk_model* m, int li) {
   const Index& ix = m->plan.index;
   if (!ix.hf_arch.empty()) o << ",\"layout\":\"hf\",\"architecture\":\"" << json_escape(ix.hf_arch) << "\"";
   if (ix.layer_end) o << ",\"layerBegin\":" << ix.layer_begin << ",\"layerEnd\":" << ix.layer_end << ",\"nLayers\":" << ix.n_layers;
+  if (m->adapter) o << ",\"adapter\":{\"path\":\"" << json_escape(m->adapter->path) << "\",\"nTensors\":" << m->adapter->pairs.size() << "}";
   o << ",\"tensors\":[";
   for (size_t i = 0; i < T.size(); ++i) {
     const DtypeInfo* di = dtype_info(pl[i].dtype);
@@ -1094,7 +1165,11 @@ std::string model_stats(kk_model* m) {
       << ",\"segs\":" << pp.segs.size() << ",\"tiles\":" << tiles << ",\"src_bytes\":" << pp.src_bytes << ",\"out_bytes\":" << pp.out_bytes
       << ",\"pool_lo\":" << lo << ",\"pool_hi\":" << hi << ",\"seconds\":" << (li < m->t_part.size() ? m->t_part[li] : 0.0) << "}";
   }
-  o << "]}";
+  o << "]";
+  if (m->adapter)
+    o << ",\"adapter\":{\"path\":\"" << json_escape(m->adapter->path) << "\",\"n_tensors\":" << m->adapter->pairs.size()
+      << ",\"n_skipped\":" << m->adapter->skipped.size() << ",\"bytes\":" << m->adapter_bytes << ",\"t_merge\":" << m->t_merge << "}";
+  o << "}";
   return o.str();
 }
 

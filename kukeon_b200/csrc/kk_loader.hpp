@@ -10,6 +10,7 @@
 #include <string>
 #include <vector>
 
+#include "kk_adapter.hpp"
 #include "kk_common.hpp"
 #include "kk_kernels.cuh"
 #include "kk_mem.hpp"
@@ -161,6 +162,11 @@ struct kk_model {
   std::atomic<uint64_t> rd_wait_ns{0}, rd_pread_ns{0}, rd_issue_ns{0}, rd_drain_ns{0};
   double t_files_open = 0, t_files_close = 0;  // of the last load: open + map, unmap + close
   uint32_t rd_threads = 0;
+  // kk_load_adapter: the LoRA adapter merged into every pool at the end of each load; the merge's device time (CUDA events, slowest device) and
+  // the bytes of its device buffer (A and B as fp32 plus the target table, per device; freed when the load returns) of the last load
+  std::unique_ptr<kk::Adapter> adapter;
+  double t_merge = 0;
+  uint64_t adapter_bytes = 0;
 };
 
 namespace kk {
@@ -168,7 +174,8 @@ namespace kk {
 kk_ctx* ctx_open(const kk_config& cfg);
 void ctx_close(kk_ctx* c);
 
-kk_model* model_load(kk_ctx* c, const std::string& path, const kk_load_opts& opts);
+// adapter_path: a PEFT LoRA adapter to merge into the pool(s) (kk_load_adapter), or empty.
+kk_model* model_load(kk_ctx* c, const std::string& path, const kk_load_opts& opts, const std::string& adapter_path = std::string());
 void model_load_part(kk_model* m);
 void model_release(kk_model* m);
 void model_peer_attach(kk_model* m, PeerKind kind, int rank, const void* handle, bool is_ipc);

@@ -107,7 +107,7 @@ ABI_SYMBOLS = [
     "kk_model_get_info", "kk_placements", "kk_model_tensor", "kk_export", "kk_export_size", "kk_pool_ptr",
     "kk_acquire", "kk_release", "kk_stats", "kk_read", "kk_checksum", "kk_stage_resident", "kk_convert_resident",
     "kk_unstage_resident", "kk_probe_hbm", "kk_probe_peer", "kk_device_identity",
-    "kk_export_fd", "kk_import_fd", "kk_import_close",
+    "kk_export_fd", "kk_import_fd", "kk_import_close", "kk_load_adapter", "kk_adapter_describe",
 ]
 
 
@@ -146,6 +146,8 @@ def lib():
     L.kk_load.argtypes = [vp, C.c_char_p, C.c_int, C.c_int, C.POINTER(vp)]
     L.kk_load_ex.argtypes = [vp, C.c_char_p, C.POINTER(KKLoadOpts), C.POINTER(vp)]
     L.kk_load_part.argtypes = [vp]
+    L.kk_load_adapter.argtypes = [vp, C.c_char_p, C.POINTER(KKLoadOpts), C.c_char_p, C.POINTER(vp)]
+    L.kk_adapter_describe.argtypes = [vp, C.c_char_p, C.POINTER(KKLoadOpts), C.c_char_p, C.c_char_p, C.c_size_t, C.POINTER(C.c_size_t)]
     L.kk_peer_attach.argtypes = [vp, C.c_int, C.c_void_p]
     L.kk_peer_detach_all.argtypes = [vp]
     L.kk_export_buffer.argtypes = [vp, C.c_int, C.c_int, C.c_void_p]
@@ -259,6 +261,21 @@ def plan_describe(path: str, mode: int = MODE_SINGLE, flags: int = 0, n_parts: i
     _check(L.kk_plan_describe(None, os.fsencode(path), C.byref(o), n_parts, chunk_bytes, None, 0, C.byref(need)))
     buf = C.create_string_buffer(need.value)
     _check(L.kk_plan_describe(None, os.fsencode(path), C.byref(o), n_parts, chunk_bytes, buf, need.value, None))
+    return json.loads(buf.value.decode("utf-8"))
+
+
+def adapter_describe(path: str, adapter: str, mode: int = MODE_SINGLE, fanout: int = FANOUT_P2P, flags: int = 0, part_index: int = 0,
+                     part_count: int = 0, layers: Optional[Sequence[int]] = None) -> dict:
+    """kk_adapter_describe: the LoRA merge a kk_load_adapter with these options would do (targets, ranks, scalings), or the error it
+    would raise.  CPU only; needs no context."""
+    L = lib()
+    o = KKLoadOpts()
+    o.mode, o.fanout, o.flags, o.part_index, o.part_count = mode, fanout, flags, part_index, part_count
+    _set_layers(o, layers)
+    need = C.c_size_t()
+    _check(L.kk_adapter_describe(None, os.fsencode(path), C.byref(o), os.fsencode(adapter), None, 0, C.byref(need)))
+    buf = C.create_string_buffer(need.value)
+    _check(L.kk_adapter_describe(None, os.fsencode(path), C.byref(o), os.fsencode(adapter), buf, need.value, None))
     return json.loads(buf.value.decode("utf-8"))
 
 
@@ -446,13 +463,17 @@ class Pool:
         self.devices = list(devices)
 
     def load(self, path: str, mode: int = MODE_SINGLE, fanout: int = FANOUT_P2P, flags: int = 0, part_index: int = 0,
-             part_count: int = 0, layers: Optional[Sequence[int]] = None) -> Model:
-        """kk_load_ex.  layers=(begin, end) loads the pipeline stage [begin, end) only, as a model of its own."""
+             part_count: int = 0, layers: Optional[Sequence[int]] = None, adapter: Optional[str] = None) -> Model:
+        """kk_load_ex.  layers=(begin, end) loads the pipeline stage [begin, end) only, as a model of its own.  adapter: a PEFT LoRA
+        adapter (directory or adapter_model.safetensors) merged into the pool(s) after the load (kk_load_adapter), a model of its own."""
         o = KKLoadOpts()
         o.mode, o.fanout, o.flags, o.part_index, o.part_count = mode, fanout, flags, part_index, part_count
         _set_layers(o, layers)
         h = C.c_void_p()
-        _check(lib().kk_load_ex(self._h, os.fsencode(path), C.byref(o), C.byref(h)))
+        if adapter is None:
+            _check(lib().kk_load_ex(self._h, os.fsencode(path), C.byref(o), C.byref(h)))
+        else:
+            _check(lib().kk_load_adapter(self._h, os.fsencode(path), C.byref(o), os.fsencode(adapter), C.byref(h)))
         return Model(self, h.value)
 
     def probe_hbm(self, device: int, kind: int = 0, nbytes: int = 4 << 30) -> float:

@@ -68,13 +68,15 @@ def Pull(path: str) -> ModelRef:
 
 
 def Load(pool: gpupool.Pool, ref: ModelRef | str, mode: int = MODE_SINGLE, fanout: int = FANOUT_P2P, flags: int = 0,
-         part_index: int = 0, part_count: int = 0, layers: Optional[Sequence[int]] = None) -> gpupool.Model:
+         part_index: int = 0, part_count: int = 0, layers: Optional[Sequence[int]] = None, adapter: Optional[str] = None) -> gpupool.Model:
     """Make the checkpoint resident in the pool(s).  Returns a refcounted Model; a second Load of the same
     checkpoint returns the same resident copy with its count bumped.  layers=(begin, end) loads only that pipeline
     stage, as a model of its own.  flags are gpupool.LOAD_*: LOAD_F16 stores every float output as fp16 instead of bf16
-    (a model apart from the bf16 load of the same file); LOAD_HF_LAYOUT loads a GGUF checkpoint under Hugging Face names and layout."""
+    (a model apart from the bf16 load of the same file); LOAD_HF_LAYOUT loads a GGUF checkpoint under Hugging Face names and layout.
+    adapter: a PEFT LoRA adapter (directory or adapter_model.safetensors) merged into the pool(s) on the GPU after the load; base + adapter
+    is a model apart from the base alone."""
     path = ref.path if isinstance(ref, ModelRef) else ref
-    return pool.load(path, mode=mode, fanout=fanout, flags=flags, part_index=part_index, part_count=part_count, layers=layers)
+    return pool.load(path, mode=mode, fanout=fanout, flags=flags, part_index=part_index, part_count=part_count, layers=layers, adapter=adapter)
 
 
 @dataclass

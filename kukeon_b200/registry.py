@@ -82,19 +82,23 @@ class Entry:
     # pipeline stage [begin, end) the pool holds; None: the whole checkpoint.  A restarted daemon reloads this stage, not the whole
     # model (which need not fit the devices).
     layers: Optional[List[int]] = None
+    # PEFT LoRA adapter merged into the pool (kk_load_adapter); None: the base checkpoint alone.  A restarted daemon reloads base + adapter.
+    adapter: Optional[str] = None
 
     def to_json(self) -> dict:
         d = dict(key=self.key, path=self.path, mode=self.mode, fileBytes=self.file_bytes, poolBytes=self.pool_bytes,
                  devices=self.devices, shards=self.shards, mounts=self.mounts)
         if self.layers is not None:
             d["layers"] = self.layers
+        if self.adapter is not None:
+            d["adapter"] = self.adapter
         return d
 
     @staticmethod
     def from_json(d: dict) -> "Entry":
         layers = d.get("layers")
         return Entry(d["key"], d["path"], d["mode"], d["fileBytes"], d["poolBytes"], list(d["devices"]), list(d["shards"]), list(d.get("mounts", [])),
-                     None if layers is None else list(layers))
+                     None if layers is None else list(layers), d.get("adapter"))
 
 
 class RegistryError(RuntimeError):
@@ -161,11 +165,11 @@ class PoolRegistry:
 
     # -- steady state --------------------------------------------------------------------------
     def record(self, key: str, path: str, mode: int, file_bytes: int, pool_bytes: int, devices: List[int], shards: List[str],
-               mount_dir: Optional[str] = None, layers: Optional[Sequence[int]] = None) -> Entry:
+               mount_dir: Optional[str] = None, layers: Optional[Sequence[int]] = None, adapter: Optional[str] = None) -> Entry:
         e = self.entries.get(key)
         if e is None:
             e = Entry(key, path, mode, file_bytes, pool_bytes, sorted(devices), shard_fingerprints(shards),
-                      layers=None if layers is None else list(layers))
+                      layers=None if layers is None else list(layers), adapter=adapter)
             self.entries[key] = e
         if mount_dir and mount_dir not in e.mounts:
             e.mounts.append(mount_dir)

@@ -11,6 +11,7 @@ Proposed schema — `models[]` on a v1beta1 ContainerSpec, next to `volumes[]` (
             mode: broadcast        # single | broadcast | scatter      (kk_mode; default single)
             devices: [0, 1]        # CUDA ordinals the agent may attach to (default: every device of the daemon's pool)
             layers: [0, 16]        # pipeline stage: only layers [begin, end) of the checkpoint (default: all of them)
+            adapter: /models/llama-3-8b-lora  # absolute host path of a PEFT LoRA adapter merged into the pool on the GPU (default: none)
             target: /run/kukeon/gpupool       # absolute container path of the read-only manifest mount (default shown)
             options: {gpt2Conv1dTranspose: false, keepF32: false, f8ToBf16: false}
 
@@ -50,6 +51,9 @@ class Err:
     ModelLayersInvalid = "model layers must be [begin, end): two non-negative integers with begin < end"
     ModelOptionUnknown = "model option is not recognized"
     ModelRegistryNotSupported = "registry references are not supported; use an absolute host path as source"
+    ModelAdapterNotAbsolute = "model adapter must be an absolute host path"
+    ModelAdapterNotFound = "model adapter does not exist on the host"
+    ModelAdapterRegistryNotSupported = "adapter registry references are not supported; use an absolute host path as adapter"
 
 
 class SchemaError(ValueError):
@@ -69,6 +73,7 @@ class ModelSpec:
     target: str = DEFAULT_TARGET
     flags: int = 0
     layers: Optional[Tuple[int, int]] = None  # pipeline stage [begin, end); None: the whole checkpoint
+    adapter: Optional[str] = None  # PEFT LoRA adapter merged on load (kk_load_adapter); None: the base checkpoint alone
 
 
 def _q(s: str) -> str:
@@ -103,6 +108,19 @@ def validate_models(models: Optional[List[dict]], stat=os.stat) -> List[ModelSpe
             raise SchemaError(Err.ModelSourceNotFound, f"model[{i}] source {_q(src)}") from None
         except OSError as e:
             raise ValueError(f"failed to stat model[{i}] source {_q(src)}: {e}") from e
+        adapter = m.get("adapter")
+        if adapter is not None:
+            adapter = str(adapter).strip()
+            if not os.path.isabs(adapter):
+                if "://" in adapter or (os.sep in adapter and not adapter.startswith(".")):
+                    raise SchemaError(Err.ModelAdapterRegistryNotSupported, f"model[{i}] adapter {_q(adapter)}")
+                raise SchemaError(Err.ModelAdapterNotAbsolute, f"model[{i}] adapter {_q(adapter)}")
+            try:
+                stat(adapter)
+            except FileNotFoundError:
+                raise SchemaError(Err.ModelAdapterNotFound, f"model[{i}] adapter {_q(adapter)}") from None
+            except OSError as e:
+                raise ValueError(f"failed to stat model[{i}] adapter {_q(adapter)}: {e}") from e
         target = str(m.get("target") or DEFAULT_TARGET).strip()
         if not os.path.isabs(target):
             raise SchemaError(Err.ModelTargetNotAbsolute, f"model[{i}] target {_q(target)}")
@@ -125,7 +143,8 @@ def validate_models(models: Optional[List[dict]], stat=os.stat) -> List[ModelSpe
                 raise SchemaError(Err.ModelOptionUnknown, f"model[{i}] option {_q(str(k))}")
             if v:
                 flags |= OPTION_FLAGS[k]
-        out.append(ModelSpec(name=name, source=src, mode=MODES[mode], devices=list(devs), target=target, flags=flags, layers=layers))
+        out.append(ModelSpec(name=name, source=src, mode=MODES[mode], devices=list(devs), target=target, flags=flags, layers=layers,
+                             adapter=adapter))
     return out
 
 
