@@ -246,6 +246,18 @@ func DeviceIdentity(ordinal int) (pciBusID, uuid string, err error) {
 	return C.GoString((*C.char)(unsafe.Pointer(&bus[0]))), C.GoString((*C.char)(unsafe.Pointer(&id[0]))), nil
 }
 
+// Derive returns the model Load(<m's path, mode, flags and layers>, adapter) returns, built from m's resident pools on the GPU instead of
+// from the checkpoint file (kk_derive_adapter).  It is a model of its own and holds no reference on m.
+func (m *Model) Derive(adapter string) (*Model, error) {
+	ca := C.CString(adapter)
+	defer C.free(unsafe.Pointer(ca))
+	d := &Model{}
+	if err := call(func() C.int { return C.kk_derive_adapter(m.h, ca, &d.h) }); err != nil {
+		return nil, err
+	}
+	return d, nil
+}
+
 func (m *Model) Acquire() error { return call(func() C.int { return C.kk_acquire(m.h) }) }
 func (m *Model) Release() error { return call(func() C.int { return C.kk_release(m.h) }) }
 

@@ -126,6 +126,13 @@ class Model {
     return v;
   }
   kk_model* handle() const { return h_; }
+  // kk_derive_adapter: the model Pool::Load(<this model's path and options>, adapter) returns, built from this model's resident pools on the
+  // GPU.  A model of its own; this one may be released at once.
+  Model Derive(const std::string& adapter) const {
+    kk_model* m = nullptr;
+    errdefs::check(kk_derive_adapter(h_, adapter.c_str(), &m));
+    return Model(m);
+  }
 
  private:
   void reset() {
@@ -218,6 +225,9 @@ inline gpupool::Model Load(gpupool::Pool& pool, const std::string& path, int mod
                            gpupool::Layers layers = {}, const std::string& adapter = std::string()) {
   return pool.Load(path, mode, KK_FANOUT_P2P, flags, layers, adapter);
 }
+
+// Derive: base + a PEFT LoRA adapter built from the resident base on the GPU, the model Load(pool, base's path, ..., adapter) returns.
+inline gpupool::Model Derive(const gpupool::Model& base, const std::string& adapter) { return base.Derive(adapter); }
 
 struct OCIMount { std::string destination, type, source; std::vector<std::string> options; };
 struct MountSpec {

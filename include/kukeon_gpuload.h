@@ -309,6 +309,22 @@ int kk_load_ex(kk_ctx* ctx, const char* path, const kk_load_opts* opts, kk_model
 int kk_load_adapter(kk_ctx* ctx, const char* path, const kk_load_opts* opts, const char* adapter_path, kk_model** out);
 int kk_adapter_describe(kk_ctx* ctx, const char* path, const kk_load_opts* opts, const char* adapter_path, char* json, size_t cap,
                         size_t* required);
+/* kk_derive_adapter: the model kk_load_adapter(ctx, path, opts, adapter_path) would return, with path and opts those `base` was loaded with,
+ * built from base's resident pool(s) instead of the checkpoint file.  Only the source of the base bytes differs:
+ *   identity  the same registry key as that load: if the model is resident the call returns it (refcount + 1) and does no work, and a later
+ *             kk_load_adapter with those arguments returns the derived model.  It holds no reference on base, which may be released at once.
+ *   model     plan, placements, kk_model_tensor, kk_model_get_info, the manifest (the "adapter" object included), kk_export / kk_export_fd,
+ *             the pool budget and kk_release are those of the kk_load_adapter model.  kk_load_part on a model derived from a KK_LOAD_DEFER
+ *             base streams the file and merges again, with an identical result.
+ *   bytes     on each local device every byte of the pool allocation outside the targets is base's byte (copied by the copy engines;
+ *             nothing crosses NVLink), and every target is the kk_load_adapter merge of base's element, bit for bit.
+ *   stats     kk_stats gains "derive": {"base_key", "t_copy", "t_merge" (CUDA events, slowest device), "t_host" (adapter read, widening and
+ *             upload, seconds)}.
+ *   refusals  all raised before any allocation, with the pool budget and the registry unchanged: every refusal of kk_load_adapter for base's
+ *             options and plan; KK_ESTATE when base is not loaded (KK_LOAD_DEFER before kk_load_part, two-stage before kk_convert_local);
+ *             KK_EINVAL when base itself carries an adapter (adapters do not stack); KK_ENOMEM past the pool budget.
+ *   locks     base's data-moving calls (kk_load_part) wait while its pools are read. */
+int kk_derive_adapter(kk_model* base, const char* adapter_path, kk_model** out);
 /* Deferred / multi-process loading: after kk_load_ex(...KK_LOAD_DEFER...) and any kk_peer_attach calls,
  * move the data.  May be called again to re-load (pools are overwritten with identical bytes). */
 int kk_load_part(kk_model* m);

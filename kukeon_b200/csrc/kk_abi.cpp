@@ -190,6 +190,17 @@ int kk_load_adapter(kk_ctx* ctx, const char* path, const kk_load_opts* opts, con
   });
 }
 
+int kk_derive_adapter(kk_model* base, const char* adapter_path, kk_model** out) {
+  return guard([&] {
+    need(base, "base");
+    need(adapter_path, "adapter_path");
+    need(out, "out");
+    *out = nullptr;
+    if (!*adapter_path) kk::fail(KK_EINVAL, "adapter_path is empty");
+    *out = kk::derive_model(base, adapter_path);
+  });
+}
+
 int kk_load_part(kk_model* m) {
   return guard([&] {
     need(m, "model");

@@ -46,9 +46,10 @@ cudaError_t launch_fill(uint8_t* dst, uint64_t nbytes, int sm_count, cudaStream_
 // One-time per-device function attribute setup (dynamic shared memory opt-in).
 cudaError_t kernels_init_device();
 
-// LoRA merge (kk_lora.cu): one CTA per tile of the n_targets targets (device table, sorted by tile_begin) over `pool`, with every A and B
-// in `adapter` as fp32.  n_tiles < 2^31.
-cudaError_t launch_lora_merge(const KKLoraTarget* targets, uint32_t n_targets, uint32_t n_tiles, const float* adapter, uint8_t* pool,
-                              cudaStream_t stream);
+// LoRA merge (kk_lora.cu): one CTA per tile of the n_targets targets (device table, sorted by tile_begin), reading the target elements of
+// pool `src` and writing them merged to the same offsets of pool `dst` (src == dst: in place), with every A and B in `adapter` as fp32.
+// Writes nothing outside the targets.  n_tiles < 2^31.
+cudaError_t launch_lora_merge(const KKLoraTarget* targets, uint32_t n_targets, uint32_t n_tiles, const float* adapter, const uint8_t* src,
+                              uint8_t* dst, cudaStream_t stream);
 
 }  // namespace kk

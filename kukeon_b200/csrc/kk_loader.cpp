@@ -535,69 +535,115 @@ void raw_fanout_launch(kk_model* m, int li, std::vector<ConvertLaunch>& out) {
   out.push_back(L);
 }
 
-// kk_load_adapter: merge the adapter into every local pool, whose bytes are all written (the load's streams have been synchronised).  One launch
-// per device over a table of that pool's targets, all enqueued before any device is waited for.  A and B (fp32) and the table live in one
-// buffer per device, freed before this returns.
-void merge_adapter(kk_model* m) {
+// The merge of m's adapter into every local pool of m, reading the target elements from the same pool of `src`: m itself (kk_load_adapter, in
+// place, the load's streams synchronised) or the base m is derived from (kk_derive_adapter, whose op_mu the caller holds).  One launch per
+// device over a table of that pool's targets.  Out of place, the bytes outside the targets are copied from src's pool by the copy engines, as
+// maximal runs on the device's copy stream, issued on every device before the adapter is read and joined to the merge's stream with an event.
+// Everything is enqueued on every device before any device is waited for.  A and B (fp32) and the table live in one buffer per device, freed
+// before this returns.
+void merge_adapter(kk_model* m, const kk_model* src) {
   const Adapter& A = *m->adapter;
-  std::vector<uint64_t> a_off, b_off;
-  const std::vector<float> host = read_adapter_f32(A, a_off, b_off);
   const size_t nl = m->pools.size();
-  std::vector<DevBuf> bufs(nl);
-  std::vector<EventSet> evs;
-  evs.reserve(nl);
-  uint64_t most = 0;
-  for (size_t li = 0; li < nl; ++li) {
+  std::vector<EventSet> cev;
+  cev.reserve(nl);
+  for (size_t li = 0; src != m && li < nl; ++li) {
     Device& dev = m->ctx->devs[li];
     const std::vector<Placement>& pl = m->plan.placement_of_part(m->shape.local_parts[li]);
-    std::vector<KKLoraTarget> T;
-    uint64_t tiles = 0;
-    for (size_t i = 0; i < A.pairs.size(); ++i) {
-      const LoraPair& p = A.pairs[i];
-      const Placement& q = pl[p.tensor];
-      KKLoraTarget t{};
-      t.w_off = q.pool_offset;
-      t.a_off = a_off[i];
-      t.b_off = b_off[i];
-      t.rows = (uint32_t)q.shape[0];
-      t.cols = (uint32_t)q.shape[1];
-      t.row0 = q.slice_dim == 0 ? (uint32_t)q.slice_begin : 0;
-      t.col0 = q.slice_dim == 1 ? (uint32_t)q.slice_begin : 0;
-      t.a_ld = (uint32_t)p.a.shape[1];
-      t.r = p.r;
-      t.s = p.s;
-      t.out = lora_out_of(q.dtype);
-      t.tile_begin = (uint32_t)tiles;
-      t.tiles_c = (t.cols + KK_LORA_TILE_C - 1) / KK_LORA_TILE_C;
-      const uint32_t n = kk_lora_tiles(t.rows, t.cols);
-      if (n == 0) continue;
-      tiles += n;
-      if (tiles >= (1ull << 31)) fail(KK_EUNSUPPORTED, "adapter: more than 2^31 merge tiles on one device");
-      T.push_back(t);
+    std::vector<std::pair<uint64_t, uint64_t>> tg;
+    for (const LoraPair& p : A.pairs) tg.push_back({pl[p.tensor].pool_offset, pl[p.tensor].pool_offset + pl[p.tensor].nbytes});
+    std::sort(tg.begin(), tg.end());
+    const uint64_t span = m->pools[li].span();  // src's pool has the same plan bytes and backing, so the same span
+    std::vector<std::pair<uint64_t, uint64_t>> runs;  // the complement of the targets in [0, span)
+    uint64_t at = 0;
+    for (auto& t : tg) {
+      if (t.first > at) runs.push_back({at, t.first});
+      at = std::max(at, t.second);
     }
-    const uint64_t tb = align_up(T.size() * sizeof(KKLoraTarget), 256), bytes = tb + host.size() * sizeof(float);
+    if (at < span) runs.push_back({at, span});
     KK_CUDA(cudaSetDevice(dev.ordinal));
-    bufs[li] = DevBuf(dev.ordinal, bytes, "the adapter");
-    if (!T.empty()) KK_CUDA(cudaMemcpy(bufs[li].get(), T.data(), T.size() * sizeof(KKLoraTarget), cudaMemcpyHostToDevice));
-    KK_CUDA(cudaMemcpy(bufs[li].get() + tb, host.data(), host.size() * sizeof(float), cudaMemcpyHostToDevice));
-    evs.emplace_back(2);
-    evs[li].create_all();
-    KK_CUDA(cudaEventRecord(evs[li][0], dev.stream));
-    KK_CUDA(launch_lora_merge(bufs[li].get<KKLoraTarget>(), (uint32_t)T.size(), (uint32_t)tiles, (const float*)(bufs[li].get() + tb),
-                              m->pools[li].ptr, dev.stream));
-    KK_CUDA(cudaEventRecord(evs[li][1], dev.stream));
-    most = std::max(most, bytes);
+    cev.emplace_back(2);
+    cev[li].create_all();
+    KK_CUDA(cudaEventRecord(cev[li][0], dev.copy_stream));
+    for (auto& r : runs)
+      KK_CUDA(cudaMemcpyAsync(m->pools[li].ptr + r.first, src->pools[li].ptr + r.first, r.second - r.first, cudaMemcpyDeviceToDevice, dev.copy_stream));
+    KK_CUDA(cudaEventRecord(cev[li][1], dev.copy_stream));
   }
-  float worst = 0.f;
-  for (size_t li = 0; li < nl; ++li) {
-    KK_CUDA(cudaSetDevice(m->ctx->devs[li].ordinal));
-    KK_CUDA(cudaStreamSynchronize(m->ctx->devs[li].stream));
-    float ms = 0.f;
-    KK_CUDA(cudaEventElapsedTime(&ms, evs[li][0], evs[li][1]));
-    worst = std::max(worst, ms);
+  try {
+    double t_host = now_s();
+    std::vector<uint64_t> a_off, b_off;
+    const std::vector<float> host = read_adapter_f32(A, a_off, b_off);
+    t_host = now_s() - t_host;
+    std::vector<DevBuf> bufs(nl);
+    std::vector<EventSet> evs;
+    evs.reserve(nl);
+    uint64_t most = 0;
+    for (size_t li = 0; li < nl; ++li) {
+      Device& dev = m->ctx->devs[li];
+      const std::vector<Placement>& pl = m->plan.placement_of_part(m->shape.local_parts[li]);
+      std::vector<KKLoraTarget> T;
+      uint64_t tiles = 0;
+      for (size_t i = 0; i < A.pairs.size(); ++i) {
+        const LoraPair& p = A.pairs[i];
+        const Placement& q = pl[p.tensor];
+        KKLoraTarget t{};
+        t.w_off = q.pool_offset;
+        t.a_off = a_off[i];
+        t.b_off = b_off[i];
+        t.rows = (uint32_t)q.shape[0];
+        t.cols = (uint32_t)q.shape[1];
+        t.row0 = q.slice_dim == 0 ? (uint32_t)q.slice_begin : 0;
+        t.col0 = q.slice_dim == 1 ? (uint32_t)q.slice_begin : 0;
+        t.a_ld = (uint32_t)p.a.shape[1];
+        t.r = p.r;
+        t.s = p.s;
+        t.out = lora_out_of(q.dtype);
+        t.tile_begin = (uint32_t)tiles;
+        t.tiles_c = (t.cols + KK_LORA_TILE_C - 1) / KK_LORA_TILE_C;
+        const uint32_t n = kk_lora_tiles(t.rows, t.cols);
+        if (n == 0) continue;
+        tiles += n;
+        if (tiles >= (1ull << 31)) fail(KK_EUNSUPPORTED, "adapter: more than 2^31 merge tiles on one device");
+        T.push_back(t);
+      }
+      const uint64_t tb = align_up(T.size() * sizeof(KKLoraTarget), 256), bytes = tb + host.size() * sizeof(float);
+      const double tu = now_s();
+      KK_CUDA(cudaSetDevice(dev.ordinal));
+      bufs[li] = DevBuf(dev.ordinal, bytes, "the adapter");
+      if (!T.empty()) KK_CUDA(cudaMemcpy(bufs[li].get(), T.data(), T.size() * sizeof(KKLoraTarget), cudaMemcpyHostToDevice));
+      KK_CUDA(cudaMemcpy(bufs[li].get() + tb, host.data(), host.size() * sizeof(float), cudaMemcpyHostToDevice));
+      t_host += now_s() - tu;
+      evs.emplace_back(2);
+      evs[li].create_all();
+      KK_CUDA(cudaEventRecord(evs[li][0], dev.stream));
+      KK_CUDA(launch_lora_merge(bufs[li].get<KKLoraTarget>(), (uint32_t)T.size(), (uint32_t)tiles, (const float*)(bufs[li].get() + tb),
+                                src->pools[li].ptr, m->pools[li].ptr, dev.stream));
+      KK_CUDA(cudaEventRecord(evs[li][1], dev.stream));
+      if (!cev.empty()) KK_CUDA(cudaStreamWaitEvent(dev.stream, cev[li][1], 0));
+      most = std::max(most, bytes);
+    }
+    float worst = 0.f, worst_copy = 0.f;
+    for (size_t li = 0; li < nl; ++li) {
+      KK_CUDA(cudaSetDevice(m->ctx->devs[li].ordinal));
+      KK_CUDA(cudaStreamSynchronize(m->ctx->devs[li].stream));
+      float ms = 0.f;
+      KK_CUDA(cudaEventElapsedTime(&ms, evs[li][0], evs[li][1]));
+      worst = std::max(worst, ms);
+      if (cev.empty()) continue;
+      KK_CUDA(cudaEventElapsedTime(&ms, cev[li][0], cev[li][1]));
+      worst_copy = std::max(worst_copy, ms);
+    }
+    m->t_merge = worst / 1e3;
+    m->t_copy = worst_copy / 1e3;
+    m->t_host = t_host;
+    m->adapter_bytes = most;
+  } catch (...) {
+    // the copies read src's pools and write m's: both must outlive them
+    for (size_t li = 0; li < cev.size(); ++li) {
+      cudaSetDevice(m->ctx->devs[li].ordinal);
+      cudaStreamSynchronize(m->ctx->devs[li].copy_stream);
+    }
+    throw;
   }
-  m->t_merge = worst / 1e3;
-  m->adapter_bytes = most;
 }
 
 // Close the peer buffers this process opened over CUDA IPC and forget every attached one.
@@ -622,6 +668,105 @@ std::string canon(const std::string& p) {
   char buf[4096];
   if (realpath(p.c_str(), buf)) return buf;
   return p;
+}
+
+// The registry key of base + adapter: the base model's key and the canonical adapter path.
+std::string adapter_key(const std::string& base_key, const std::string& adapter_path) { return base_key + "|a" + canon(adapter_path); }
+
+// The model registered under `key`, refcount + 1, once no load of it is in flight (found = true); or a new model registered there, loading,
+// refcount 1, that the caller builds and then publishes or abandons.
+kk_model* claim_key(kk_ctx* c, const std::string& key, bool& found) {
+  std::unique_lock<std::mutex> lk(c->mu);
+  for (;;) {
+    auto it = c->models.find(key);
+    if (it == c->models.end()) break;
+    if (it->second->loading) { c->cv.wait(lk); continue; }
+    it->second->refcount++;
+    found = true;
+    return it->second;
+  }
+  found = false;
+  kk_model* m = new kk_model;
+  m->ctx = c;
+  m->key = key;
+  m->refcount = 1;
+  m->loading = true;
+  c->models[key] = m;
+  return m;
+}
+
+void publish(kk_model* m) {
+  {
+    std::lock_guard<std::mutex> g(m->ctx->mu);
+    m->loading = false;
+  }
+  m->ctx->cv.notify_all();
+}
+
+// A claimed model whose build failed: unregistered, waiters woken (they claim the key again), its memory and budget returned.
+void abandon(kk_model* m) {
+  kk_ctx* c = m->ctx;
+  {
+    std::lock_guard<std::mutex> g(c->mu);
+    c->models.erase(m->key);
+  }
+  c->cv.notify_all();
+  destroy_model(m);
+}
+
+// The pools of m's plan and shape on every local device, each reserved on the device's pool budget first (KK_ENOMEM past it), and every
+// device's copy of the concatenated segment table.
+void alloc_pools(kk_model* m) {
+  kk_ctx* c = m->ctx;
+  const LoadShape& S = m->shape;
+  std::vector<KKSeg> all;
+  for (auto& pp : m->plan.parts) all.insert(all.end(), pp.segs.begin(), pp.segs.end());
+  const size_t nl = S.local_parts.size();
+  m->pools = std::vector<Pool>(nl);
+  m->d_segs.resize(nl);
+  if (S.order == LoadOrder::kNvls) {
+    std::string why;
+    if (!plan_allows_multimem(m->plan, &why)) fail(KK_EUNSUPPORTED, "fan-out NVLS: %s", why.c_str());
+    std::vector<int> ords;
+    for (auto& d : c->devs) ords.push_back(d.ordinal);
+    KK_CUDA(cudaSetDevice(ords[0]));  // the driver entry points below want a current context on the calling thread
+    m->nvls.reset(new NvlsPools);
+    m->nvls->create(ords, m->plan.pool_bytes_of_part(0));
+  }
+  for (size_t li = 0; li < nl; ++li) {
+    Device& d = c->devs[li];
+    KK_CUDA(cudaSetDevice(d.ordinal));
+    const uint64_t pb = m->plan.pool_bytes_of_part(S.local_parts[li]);
+    Pool& pool = m->pools[li];
+    {
+      std::lock_guard<std::mutex> g(c->mu);
+      if (c->cfg.pool_bytes_per_device && d.pool_in_use + pb > c->cfg.pool_bytes_per_device)
+        fail(KK_ENOMEM, "device %d: pool budget exceeded (%llu in use + %llu > %llu)", d.ordinal, (unsigned long long)d.pool_in_use,
+             (unsigned long long)pb, (unsigned long long)c->cfg.pool_bytes_per_device);
+      d.pool_in_use += pb;
+      pool.bytes = pb;
+      pool.ctx = c;
+      pool.dev = &d;
+    }
+    if (m->nvls) {
+      pool.ptr = m->nvls->pool(li);  // already allocated, bound and mapped
+    } else if (c->cfg.flags & KK_CFG_VMM_POOLS) {
+      // cuMemCreate memory: exported as a POSIX fd (kk_export_fd) that another process maps READ-ONLY, which a cudaIpcMemHandle cannot offer.
+      // Mapped read-write here for this device and, in a peer-enabled context, for the other devices (fan-out stores land in it).
+      std::vector<int> acc;
+      if (c->peer_ok)
+        for (auto& dv : c->devs) acc.push_back(dv.ordinal);
+      pool.vmm.reset(new VmmAlloc);
+      pool.vmm->create(d.ordinal, pb, acc);
+      pool.ptr = pool.vmm->ptr();
+    } else {
+      // whole 2 MiB multiples: the driver sub-allocates smaller requests out of shared 2 MiB blocks, and an IPC handle maps the whole block —
+      // a pool that owns its blocks outright cannot expose a neighbouring allocation through its handle (round-1 review)
+      pool.mem = DevBuf(d.ordinal, align_up(pb ? pb : 1, 2u << 20), "the pool");
+      pool.ptr = pool.mem.get();
+    }
+    m->d_segs[li] = upload_segs(d.ordinal, all);
+  }
 }
 
 }  // namespace
@@ -696,6 +841,7 @@ kk_ctx* ctx_open(const kk_config& cfg_in) {
           KK_CUDA(kernels_init_device());
           d.kernels_ready = true;
           KK_CUDA(cudaStreamCreateWithFlags(&d.stream, cudaStreamNonBlocking));
+          KK_CUDA(cudaStreamCreateWithFlags(&d.copy_stream, cudaStreamNonBlocking));
           d.sched = DevBuf(d.ordinal, 256, "the scheduling words");
           KK_CUDA(cudaMemset(d.sched.get(), 0, 256));
           d.numa_cpus = numa_cpus_of_device(d.ordinal);
@@ -772,6 +918,7 @@ void ctx_close(kk_ctx* c) {
       if (rd.stream) cudaStreamDestroy(rd.stream);
     }
     if (d.stream) cudaStreamDestroy(d.stream);
+    if (d.copy_stream) cudaStreamDestroy(d.copy_stream);
   }
   delete c;  // the device buffers go with it
 }
@@ -811,7 +958,7 @@ static void do_load(kk_model* m) {
   const double tc = now_s();
   fds.cleanup();  // part of the load: unmapping a checkpoint-sized mapping is not free
   m->t_files_close = now_s() - tc;
-  if (m->adapter) merge_adapter(m);  // every pool is complete: no load shape that merges has a second stage or a peer's stores still to come
+  if (m->adapter) merge_adapter(m, m);  // every pool is complete: no load shape that merges has a second stage or a peer's stores still to come
   m->t_load = now_s() - t0;
   m->n_loads++;
   std::lock_guard<std::mutex> g(m->ctx->mu);
@@ -832,27 +979,14 @@ kk_model* model_load(kk_ctx* c, const std::string& path, const kk_load_opts& opt
   std::ostringstream ks;
   ks << canon(path) << "|m" << opts.mode << "|f" << opts.fanout << "|x" << (opts.flags & ~KK_LOAD_DEFER) << "|p" << opts.part_index << "/" << opts.part_count
      << "|l" << opts.layer_begin << ":" << opts.layer_end;
-  if (!adapter_path.empty()) ks << "|a" << canon(adapter_path);
-  const std::string key = ks.str();
+  const std::string key = adapter_path.empty() ? ks.str() : adapter_key(ks.str(), adapter_path);
 
-  kk_model* m = nullptr;
-  {
-    std::unique_lock<std::mutex> lk(c->mu);
-    for (;;) {
-      auto it = c->models.find(key);
-      if (it == c->models.end()) break;
-      if (it->second->loading) { c->cv.wait(lk); continue; }
-      it->second->refcount++;
-      return it->second;
-    }
-    m = new kk_model;
-    m->ctx = c;
-    m->key = key;
-    m->shape = std::move(shape);
-    m->refcount = 1;
-    m->loading = true;
-    c->models[key] = m;
-  }
+  bool found = false;
+  kk_model* m = claim_key(c, key, found);
+  if (found) return m;
+  m->path = path;
+  m->opts = opts;
+  m->shape = std::move(shape);
   const LoadShape& S = m->shape;
   try {
     double t0 = now_s();
@@ -863,55 +997,7 @@ kk_model* model_load(kk_ctx* c, const std::string& path, const kk_load_opts& opt
     if (!adapter_path.empty()) m->adapter.reset(new Adapter(match_adapter(adapter_path, path, opts.flags, m->plan)));
     m->t_plan = now_s() - t0;
     t0 = now_s();
-    // concatenated segment table of all parts
-    std::vector<KKSeg> all;
-    for (auto& pp : m->plan.parts) all.insert(all.end(), pp.segs.begin(), pp.segs.end());
-    const size_t nl = S.local_parts.size();
-    m->pools = std::vector<Pool>(nl);
-    m->d_segs.resize(nl);
-    if (S.order == LoadOrder::kNvls) {
-      std::string why;
-      if (!plan_allows_multimem(m->plan, &why)) fail(KK_EUNSUPPORTED, "fan-out NVLS: %s", why.c_str());
-      std::vector<int> ords;
-      for (auto& d : c->devs) ords.push_back(d.ordinal);
-      KK_CUDA(cudaSetDevice(ords[0]));  // the driver entry points below want a current context on the calling thread
-      m->nvls.reset(new NvlsPools);
-      m->nvls->create(ords, m->plan.pool_bytes_of_part(0));
-    }
-    for (size_t li = 0; li < nl; ++li) {
-      Device& d = c->devs[li];
-      KK_CUDA(cudaSetDevice(d.ordinal));
-      const uint64_t pb = m->plan.pool_bytes_of_part(S.local_parts[li]);
-      Pool& pool = m->pools[li];
-      {
-        std::lock_guard<std::mutex> g(c->mu);
-        if (c->cfg.pool_bytes_per_device && d.pool_in_use + pb > c->cfg.pool_bytes_per_device)
-          fail(KK_ENOMEM, "device %d: pool budget exceeded (%llu in use + %llu > %llu)", d.ordinal, (unsigned long long)d.pool_in_use,
-               (unsigned long long)pb, (unsigned long long)c->cfg.pool_bytes_per_device);
-        d.pool_in_use += pb;
-        pool.bytes = pb;
-        pool.ctx = c;
-        pool.dev = &d;
-      }
-      if (m->nvls) {
-        pool.ptr = m->nvls->pool(li);  // already allocated, bound and mapped
-      } else if (c->cfg.flags & KK_CFG_VMM_POOLS) {
-        // cuMemCreate memory: exported as a POSIX fd (kk_export_fd) that another process maps READ-ONLY, which a cudaIpcMemHandle cannot offer.
-        // Mapped read-write here for this device and, in a peer-enabled context, for the other devices (fan-out stores land in it).
-        std::vector<int> acc;
-        if (c->peer_ok)
-          for (auto& dv : c->devs) acc.push_back(dv.ordinal);
-        pool.vmm.reset(new VmmAlloc);
-        pool.vmm->create(d.ordinal, pb, acc);
-        pool.ptr = pool.vmm->ptr();
-      } else {
-        // whole 2 MiB multiples: the driver sub-allocates smaller requests out of shared 2 MiB blocks, and an IPC handle maps the whole block —
-        // a pool that owns its blocks outright cannot expose a neighbouring allocation through its handle (round-1 review)
-        pool.mem = DevBuf(d.ordinal, align_up(pb ? pb : 1, 2u << 20), "the pool");
-        pool.ptr = pool.mem.get();
-      }
-      m->d_segs[li] = upload_segs(d.ordinal, all);
-    }
+    alloc_pools(m);
     if (S.order == LoadOrder::kRaw) setup_raw(m);
     if (S.order == LoadOrder::kPull) {
       m->part_range.assign((size_t)m->plan.n_parts, {0, 0});
@@ -931,19 +1017,50 @@ kk_model* model_load(kk_ctx* c, const std::string& path, const kk_load_opts& opt
       if (S.order == LoadOrder::kRaw && !S.two_stage) m->images.clear();  // the gathered file bytes are not needed once the pools are built
     }
   } catch (...) {
-    {
-      std::lock_guard<std::mutex> g(c->mu);
-      c->models.erase(key);
-    }
-    c->cv.notify_all();
-    destroy_model(m);
+    abandon(m);
     throw;
   }
+  publish(m);
+  return m;
+}
+
+kk_model* derive_model(kk_model* base, const std::string& adapter_path) {
+  kk_ctx* c = base->ctx;
+  check_adapter_opts(base->opts);  // before the state check: a load shape that cannot merge never will
   {
     std::lock_guard<std::mutex> g(c->mu);
-    m->loading = false;
+    if (base->adapter) fail(KK_EINVAL, "kk_derive_adapter: the base model carries an adapter already (adapters do not stack)");
+    if (!base->loaded) fail(KK_ESTATE, "kk_derive_adapter: the base model is not loaded (kk_load_part / kk_convert_local first)");
   }
-  c->cv.notify_all();
+  const double t0 = now_s();
+  bool found = false;
+  kk_model* m = claim_key(c, adapter_key(base->key, adapter_path), found);
+  if (found) return m;
+  try {
+    // the base's path, options, plan and shape never change once it is published
+    m->path = base->path;
+    m->opts = base->opts;
+    m->shape = base->shape;
+    m->plan = base->plan;
+    m->base_key = base->key;
+    m->adapter.reset(new Adapter(match_adapter(adapter_path, m->path, m->opts.flags, m->plan)));
+    m->t_plan = now_s() - t0;
+    const double ta = now_s();
+    alloc_pools(m);
+    // a deferred RAW model keeps its raw image for kk_load_part, as the load of base + adapter does; other shapes that merge have none
+    if (m->shape.order == LoadOrder::kRaw && (m->opts.flags & KK_LOAD_DEFER)) setup_raw(m);
+    m->t_alloc = now_s() - ta;
+    {
+      std::lock_guard<std::mutex> op(base->op_mu);  // a kk_load_part of the base must not rewrite its pools under the copy
+      merge_adapter(m, base);
+    }
+    std::lock_guard<std::mutex> g(c->mu);
+    m->loaded = true;
+  } catch (...) {
+    abandon(m);
+    throw;
+  }
+  publish(m);
   return m;
 }
 
@@ -1169,6 +1286,9 @@ std::string model_stats(kk_model* m) {
   if (m->adapter)
     o << ",\"adapter\":{\"path\":\"" << json_escape(m->adapter->path) << "\",\"n_tensors\":" << m->adapter->pairs.size()
       << ",\"n_skipped\":" << m->adapter->skipped.size() << ",\"bytes\":" << m->adapter_bytes << ",\"t_merge\":" << m->t_merge << "}";
+  if (!m->base_key.empty())
+    o << ",\"derive\":{\"base_key\":\"" << json_escape(m->base_key) << "\",\"t_copy\":" << m->t_copy << ",\"t_merge\":" << m->t_merge
+      << ",\"t_host\":" << m->t_host << "}";
   o << "}";
   return o.str();
 }

@@ -59,6 +59,7 @@ struct Device {
   int sm_count = 0;
   std::vector<Reader> readers;
   cudaStream_t stream = nullptr;  // resident launches, checksum, misc
+  cudaStream_t copy_stream = nullptr;  // kk_derive_adapter: the pool bytes outside the targets, copied while the merge runs on `stream`
   DevBuf sched;                   // tile-scheduling counters every launch on `stream` needs (first 8 of 256 zeroed bytes)
   std::unique_ptr<std::mutex> sum_mu{new std::mutex};  // kk_checksum's accumulator is the 8 bytes at sched + 32 words: no cudaMalloc / cudaFree per call
   uint64_t pool_in_use = 0;
@@ -100,6 +101,7 @@ struct Pool {
   kk_ctx* ctx = nullptr;          // set once `bytes` are reserved on dev->pool_in_use
   Device* dev = nullptr;
   bool is_nvls() const { return ptr && !mem && !vmm; }
+  uint64_t span() const { return mem ? mem.bytes() : vmm ? vmm->bytes() : bytes; }  // the bytes behind ptr: plan bytes and the allocation's tail
   Pool() = default;
   Pool(const Pool&) = delete;
   ~Pool();
@@ -120,6 +122,8 @@ struct kk_ctx {
 struct kk_model {
   kk_ctx* ctx = nullptr;
   std::string key;
+  std::string path;   // the checkpoint and the options it was loaded with (part_count <= 1 normalised to 1 / 0)
+  kk_load_opts opts{};
   kk::Plan plan;
   kk::LoadShape shape;  // local device li (every per-device vector below) is ctx->devs[li]
   // KK_FANOUT_NVLS (one process, >= 2 devices): per-device VMM allocations bound to one multicast object; the pools alias them, and this is
@@ -167,6 +171,10 @@ struct kk_model {
   std::unique_ptr<kk::Adapter> adapter;
   double t_merge = 0;
   uint64_t adapter_bytes = 0;
+  // kk_derive_adapter: the key of the base model the pools were derived from (empty for a model loaded from its file), and the derive's copy
+  // of the bytes outside the targets (CUDA events, slowest device) and host time (adapter read, widening and upload)
+  std::string base_key;
+  double t_copy = 0, t_host = 0;
 };
 
 namespace kk {
@@ -176,6 +184,8 @@ void ctx_close(kk_ctx* c);
 
 // adapter_path: a PEFT LoRA adapter to merge into the pool(s) (kk_load_adapter), or empty.
 kk_model* model_load(kk_ctx* c, const std::string& path, const kk_load_opts& opts, const std::string& adapter_path = std::string());
+// kk_derive_adapter: the model model_load(base's path, base's opts, adapter_path) returns, its pools built from base's pools on the GPU.
+kk_model* derive_model(kk_model* base, const std::string& adapter_path);
 void model_load_part(kk_model* m);
 void model_release(kk_model* m);
 void model_peer_attach(kk_model* m, PeerKind kind, int rank, const void* handle, bool is_ipc);

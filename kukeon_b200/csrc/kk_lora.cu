@@ -1,5 +1,6 @@
-// kk_lora_merge_kernel: the LoRA merge of kk_load_adapter over one device's pool (the arithmetic and the tile walk: kk_lora.cuh).
-// One CTA per tile of every target in the table; the pool is read and written once, A and B come from L2 through shared memory.
+// kk_lora_merge_kernel: the LoRA merge of kk_load_adapter (in place) and kk_derive_adapter (out of place) over one device's pool (the arithmetic
+// and the tile walk: kk_lora.cuh).  One CTA per tile of every target in the table; every target element is read from `src` and written to `dst`
+// once, A and B come from L2 through shared memory.  src and dst are not __restrict__: in place they are the same pool.
 #include <cuda_runtime.h>
 
 #include "kk_kernels.cuh"
@@ -10,7 +11,7 @@ namespace kk {
 namespace {
 
 __global__ void __launch_bounds__(KK_LORA_THREADS) kk_lora_merge_kernel(const KKLoraTarget* __restrict__ T, uint32_t n_targets,
-                                                                        const float* __restrict__ ad, uint8_t* __restrict__ pool) {
+                                                                        const float* __restrict__ ad, const uint8_t* src, uint8_t* dst) {
   __shared__ float Bs[KK_LORA_TILE_R * KK_LORA_BS_LD];
   __shared__ __align__(16) float As[KK_LORA_KSTEP * KK_LORA_TILE_C];
   const uint32_t tile = blockIdx.x, tid = threadIdx.x;
@@ -28,15 +29,15 @@ __global__ void __launch_bounds__(KK_LORA_THREADS) kk_lora_merge_kernel(const KK
     const uint32_t kn = t.r - k0 < KK_LORA_KSTEP ? t.r - k0 : KK_LORA_KSTEP;
     kk_lora_fma_step(Bs, As, kn, tid, acc);
   }
-  kk_lora_store(t, g, pool, tid, acc);
+  kk_lora_store(t, g, src, dst, tid, acc);
 }
 
 }  // namespace
 
-cudaError_t launch_lora_merge(const KKLoraTarget* targets, uint32_t n_targets, uint32_t n_tiles, const float* adapter, uint8_t* pool,
-                              cudaStream_t stream) {
+cudaError_t launch_lora_merge(const KKLoraTarget* targets, uint32_t n_targets, uint32_t n_tiles, const float* adapter, const uint8_t* src,
+                              uint8_t* dst, cudaStream_t stream) {
   if (n_tiles == 0) return cudaSuccess;
-  kk_lora_merge_kernel<<<n_tiles, KK_LORA_THREADS, 0, stream>>>(targets, n_targets, adapter, pool);
+  kk_lora_merge_kernel<<<n_tiles, KK_LORA_THREADS, 0, stream>>>(targets, n_targets, adapter, src, dst);
   return cudaGetLastError();
 }
 

@@ -1,4 +1,4 @@
-// LoRA merge (kk_load_adapter): W += s * B.A over finished pool tensors, shared by kk_lora_merge_kernel (kk_lora.cu) and its CPU
+// LoRA merge (kk_load_adapter, kk_derive_adapter): W += s * B.A over finished pool tensors, shared by kk_lora_merge_kernel (kk_lora.cu) and its CPU
 // replay (tests/emul/kk_lora_emul.cpp).  Everything here is KK_HD and touches memory only through the pointers it is given.
 //
 // Per element (i, j) of a target, in the coordinates of the full tensor:
@@ -177,9 +177,12 @@ static inline KK_HD void kk_lora_fma_step(const float* Bs, const float* As, uint
   }
 }
 
-// Step 3, thread `tid`: read its outputs' pool elements, merge and write them back.  Whole 16-byte vectors where the row has them, single
-// elements at the right edge and in rows that are not 16-byte multiples; nothing outside the target.
-static inline KK_HD void kk_lora_store(const KKLoraTarget& t, KKLoraTile g, uint8_t* pool, uint32_t tid, const float acc[KK_LORA_TM][KK_LORA_TN]) {
+// Step 3, thread `tid`: read its outputs' elements from the pool `src`, merge them and write them to the same offsets of the pool `dst`.  Whole
+// 16-byte vectors where the row has them, single elements at the right edge and in rows that are not 16-byte multiples; nothing outside the
+// target.  src == dst merges in place (kk_load_adapter), src != dst out of place (kk_derive_adapter): each element is read and then written by
+// the same thread, so the two may alias.
+static inline KK_HD void kk_lora_store(const KKLoraTarget& t, KKLoraTile g, const uint8_t* src, uint8_t* dst, uint32_t tid,
+                                       const float acc[KK_LORA_TM][KK_LORA_TN]) {
   const uint32_t ty = tid / (KK_LORA_TILE_C / KK_LORA_TN), tx = tid % (KK_LORA_TILE_C / KK_LORA_TN);
   const uint32_t es = t.out == KK_LORA_F32 ? 4u : 2u;
   const uint32_t j0 = g.j0 + tx * KK_LORA_TN;
@@ -189,9 +192,11 @@ static inline KK_HD void kk_lora_store(const KKLoraTarget& t, KKLoraTile g, uint
   for (uint32_t ii = 0; ii < KK_LORA_TM; ++ii) {
     const uint32_t i = g.i0 + ty * KK_LORA_TM + ii;
     if (i >= t.rows) break;
-    uint8_t* row = pool + t.w_off + ((uint64_t)i * t.cols + j0) * es;
+    const uint64_t at = t.w_off + ((uint64_t)i * t.cols + j0) * es;
+    const uint8_t* in = src + at;
+    uint8_t* row = dst + at;
     if (vec && es == 2) {
-      KKLoraVec v = *(const KKLoraVec*)row;
+      KKLoraVec v = *(const KKLoraVec*)in;
       KK_LORA_UNROLL
       for (uint32_t q = 0; q < 4; ++q) {
         const uint32_t lo = kk_lora_merge16((uint16_t)(v.w[q] & 0xFFFFu), acc[ii][2 * q], t.s, t.out);
@@ -202,26 +207,30 @@ static inline KK_HD void kk_lora_store(const KKLoraTarget& t, KKLoraTile g, uint
     } else if (vec) {
       KK_LORA_UNROLL
       for (uint32_t h = 0; h < 2; ++h) {
-        KKLoraVec v = *(const KKLoraVec*)(row + 16 * h);
+        KKLoraVec v = *(const KKLoraVec*)(in + 16 * h);
         KK_LORA_UNROLL
         for (uint32_t q = 0; q < 4; ++q) v.w[q] = kk_lora_merge32(v.w[q], acc[ii][4 * h + q], t.s);
         *(KKLoraVec*)(row + 16 * h) = v;
       }
     } else {
       for (uint32_t jj = 0; jj < KK_LORA_TN && j0 + jj < t.cols; ++jj) {
-        uint8_t* e = row + jj * es;
         if (es == 2) {
           uint16_t w;
-          memcpy(&w, e, 2);
+          memcpy(&w, in + jj * 2, 2);
           w = kk_lora_merge16(w, acc[ii][jj], t.s, t.out);
-          memcpy(e, &w, 2);
+          memcpy(row + jj * 2, &w, 2);
         } else {
           uint32_t w;
-          memcpy(&w, e, 4);
+          memcpy(&w, in + jj * 4, 4);
           w = kk_lora_merge32(w, acc[ii][jj], t.s);
-          memcpy(e, &w, 4);
+          memcpy(row + jj * 4, &w, 4);
         }
       }
     }
   }
+}
+
+// Step 3 in place: src == dst == pool.
+static inline KK_HD void kk_lora_store(const KKLoraTarget& t, KKLoraTile g, uint8_t* pool, uint32_t tid, const float acc[KK_LORA_TM][KK_LORA_TN]) {
+  kk_lora_store(t, g, pool, pool, tid, acc);
 }

@@ -108,6 +108,7 @@ ABI_SYMBOLS = [
     "kk_acquire", "kk_release", "kk_stats", "kk_read", "kk_checksum", "kk_stage_resident", "kk_convert_resident",
     "kk_unstage_resident", "kk_probe_hbm", "kk_probe_peer", "kk_device_identity",
     "kk_export_fd", "kk_import_fd", "kk_import_close", "kk_load_adapter", "kk_adapter_describe",
+    "kk_derive_adapter",
 ]
 
 
@@ -148,6 +149,7 @@ def lib():
     L.kk_load_part.argtypes = [vp]
     L.kk_load_adapter.argtypes = [vp, C.c_char_p, C.POINTER(KKLoadOpts), C.c_char_p, C.POINTER(vp)]
     L.kk_adapter_describe.argtypes = [vp, C.c_char_p, C.POINTER(KKLoadOpts), C.c_char_p, C.c_char_p, C.c_size_t, C.POINTER(C.c_size_t)]
+    L.kk_derive_adapter.argtypes = [vp, C.c_char_p, C.POINTER(vp)]
     L.kk_peer_attach.argtypes = [vp, C.c_int, C.c_void_p]
     L.kk_peer_detach_all.argtypes = [vp]
     L.kk_export_buffer.argtypes = [vp, C.c_int, C.c_int, C.c_void_p]
@@ -402,6 +404,13 @@ class Model:
 
     def load_part(self) -> None:
         _check(lib().kk_load_part(self._h))
+
+    def derive(self, adapter: str) -> "Model":
+        """kk_derive_adapter: the model Pool.load(<this model's path and options>, adapter=adapter) returns, its pools built from this
+        model's resident pools on the GPU instead of from the checkpoint file.  A model of its own; this one may be released at once."""
+        h = C.c_void_p()
+        _check(lib().kk_derive_adapter(self._h, os.fsencode(adapter), C.byref(h)))
+        return Model(self._pool, h.value)
 
     # -- verification / measurement -----------------------------------------------------------
     def read(self, device: int, offset: int, nbytes: int):

@@ -79,6 +79,12 @@ def Load(pool: gpupool.Pool, ref: ModelRef | str, mode: int = MODE_SINGLE, fanou
     return pool.load(path, mode=mode, fanout=fanout, flags=flags, part_index=part_index, part_count=part_count, layers=layers, adapter=adapter)
 
 
+def Derive(model: gpupool.Model, adapter: str) -> gpupool.Model:
+    """Base + a PEFT LoRA adapter without reading the checkpoint again: the model Load(<model's path and options>, adapter=adapter)
+    returns, built from the resident base's pool(s) on the GPU (kk_derive_adapter).  A model of its own; `model` may be released at once."""
+    return model.derive(adapter)
+
+
 @dataclass
 class MountSpec:
     """What a `ctr.WithGPUWeights(...)` BuildOption would append to the container's OCI spec."""
